@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — llama-bench-shaped measurement of the quantized mat-mul hot path on B200.
+"""bench.py — llama-bench-shaped measurement of the quantized mat-mul hot path on H100.
 
 Workload (BASELINE.json configs[1]): Llama-3-8B, pure IQ4_NL (`llama-quantize --pure`), synthetic random-init weights.
 One "step" = one pass of the hot path over one batch:
   * tg128: ONE token (n_batch = 1) through every MUL_MAT of the model, in graph order with real data dependencies:
            32 x [ QKV (one multi-tensor mat-vec launch) -> wo -> fused up/gate/SiLU -> ffn_down ] -> output head.
            129 launches of our k_mmvq kernel and nothing else (attention/norm/rope are NOT the hot path and are not run;
-           the q projection is fed straight to wo so the chain keeps the dependency structure).
-  * pp512: the same matrices with n_batch = 512 through the tcgen05 GEMM path (head on the last token only,
+           the q projection is fed straight to wo so the chain keeps the dependency structure; on one GPU ffn_down adds into a residual
+           stream through its bias operand, see Model).
+  * pp512: the same matrices with n_batch = 512 through the wgmma GEMM path (head on the last token only,
            as llama-bench does); the SiLU*mul glue between up/gate and down is a torch elementwise op.
-Weights live in HBM in the plane layout (uploaded through the C-ABI repack); 4.2 GB of weights per pass >> 126 MB L2,
+Weights live in HBM in the plane layout (uploaded through the C-ABI repack); 4.2 GB of weights per pass >> 50 MB L2,
 so every timed iteration streams from HBM ("inputs larger than L2").
 
 value  = tok/s with inputs already resident in HBM (CUDA-graph replay of the step, CUDA-event timed, max over ranks)
@@ -18,6 +19,9 @@ N > 1  = the fork's "split mode graph" tensor parallelism: QKV/up/gate row-shard
 
 --impl reference times the reference's own CPU IQK path (oracle/_ref, the unmodified ggml CPU backend) on a bounded
 sample of the same workload (one transformer layer's mat-muls), scaled to the whole token.
+
+--dump-outputs DIR writes, after the timed steps, what each timed path returned in its last step as DIR/<name>.npy (float32): the inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -36,6 +40,7 @@ sys.path.insert(0, ROOT)
 
 # Llama-3-8B (SURVEY.md §8): per-layer matmul shapes (M x K)
 N_EMBD, N_FF, N_LAYER, N_VOCAB, N_KV_DIM = 4096, 14336, 32, 128256, 1024
+FFN_BRANCH_SCALE = 0.2          # gain of ffn_down on the residual stream (see Model)
 IQ4_NL = 20
 
 
@@ -50,7 +55,7 @@ def model_flops_pp(n_tokens, n_layer=N_LAYER):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index=0):
@@ -137,8 +142,13 @@ class Model:
         gen = torch.Generator(device="cuda")
         gen.manual_seed(seed + rank)
         # unit-gain weights (IQ4_NL codebook rms ~ 70).  There is no norm between the layers of this MUL_MAT-only skeleton and silu(g)*u makes the
-        # magnitude map quadratic, so the values contract towards 0 over the layers instead of overflowing the fp16 scale of q8_1
-        s_e, s_f = 1.0 / (70.0 * N_EMBD ** 0.5), 1.0 / (70.0 * N_FF ** 0.5)
+        # FFN branch quadratic in its input: a plain chain contracts to exact zeros within ~8 layers.  One GPU therefore carries a residual stream,
+        # x_{l+1} = x_l + ffn_down(...), with ffn_down scaled by FFN_BRANCH_SCALE so that the stream stays O(1) over 32 layers (rms ~1.2 at the end)
+        # and the outputs say something about the kernels.  The tensor-parallel shards keep the plain chain (their ffn_down partials are reduced
+        # inside the next kernel, where no residual add exists), so their outputs are zeros.
+        self.residual = tp == 1
+        self.hidden = None              # the hidden state after the last layer, set by every step
+        s_e, s_f = 1.0 / (70.0 * N_EMBD ** 0.5), 1.0 / (70.0 * N_FF ** 0.5) * (FFN_BRANCH_SCALE if self.residual else 1.0)
         # mix = "default": what `llama-quantize model IQ4_NL` produces WITHOUT --pure on this GQA model (src/llama-quantize.cpp:617-621, 739-745, 385-388):
         # attn_v -> IQ5_K, ffn_down of the first n_layer/8 layers -> Q5_K, output.weight -> Q6_K, everything else IQ4_NL
         self.mix = mix
@@ -157,9 +167,9 @@ class Model:
         self.bf16_reduce = False
         if tp > 1 and collective and os.environ.get("B200Q_NCCL_REDUCE", "0") != "1":
             self.reducer = be.NvlsReducer(512 * N_EMBD)
-            # decode: the reduce fused into the mat-vecs (tagged-slot exchange) wins at 2 ranks (595-631 vs 574 tok/s) but its cost grows with the number
-            # of ranks (+4.5 us per exchange at N = 2, +9.5 us at N = 4: 511-532 tok/s), while the one-shot reduce kernel's rendezvous did not grow with N
-            # in round 1 -> more than 2 ranks use the separate reduce kernel unless B200Q_TP_FUSED says otherwise (profiles/r2_tp_timeline.md)
+            # decode: the reduce fused into the mat-vecs (tagged-slot exchange) saves the reduce launches, but its exchange cost grows with the number
+            # of ranks while the one-shot reduce kernel's rendezvous does not -> more than 2 ranks use the separate reduce kernel unless
+            # B200Q_TP_FUSED says otherwise (not measured on H100)
             self.fused_tp = self.reducer.ok and os.environ.get("B200Q_TP_FUSED", "1" if tp <= 2 else "0") == "1"
             self.bf16_reduce = self.reducer.ok and os.environ.get("B200Q_TP_BF16_REDUCE", "1") == "1"
             self.launches_tg += 2 * n_layer if (self.reducer.ok and not self.fused_tp) else 0
@@ -175,6 +185,7 @@ class Model:
         self.g = f(n, N_FF // tp) if n > 8 else None
         b = lambda *s: t.empty(s, dtype=t.bfloat16, device="cuda")
         self.xb, self.qb, self.hb, self.ab = (b(n, N_EMBD), b(n, N_EMBD // tp), b(n, N_EMBD), b(n, N_FF // tp)) if n > 8 else (None,) * 4
+        self.res = (f(n, N_EMBD), f(n, N_EMBD)) if self.residual else None      # the residual stream, alternating between layers
 
     def allreduce(self, t):
         if self.tp > 1:
@@ -199,6 +210,13 @@ class Model:
             be.mul_mat_vec_tp([self.head], None, [self.logits], r, reduce_in=True)
         else:               # (correctness gate) a consumer that only materialises the reduced vector
             be.mul_mat_vec_tp([self.layers[0]["wq"]], None, [self.q], r, reduce_in=True)
+        self.hidden = None          # exists only as the reducer's tagged slots: outputs() rebuilds it
+
+    def outputs(self):
+        """What the last step returned: this rank's logits (last token) and the hidden state after the last layer.  Call after the timed
+        steps: on the fused tensor-parallel decode path the hidden state is rebuilt from the reducer's slots, which synchronises."""
+        hidden = self.hidden if self.hidden is not None else self.reducer.reduced_view(N_EMBD)[None, :]
+        return {"logits": self.logits, "hidden": hidden}
 
     def step_tg(self, with_head=True):
         be = self.be
@@ -222,8 +240,13 @@ class Model:
                 N = self.layers[li + 1]; pf([N["wq"], N["wk"], N["wv"]])
             elif with_head:
                 pf([self.head])
-            be.mul_mat(L["down"], self.a, out=self.x2, q8_in=self.q8a); self.allreduce(self.x2)
-            x = self.x2
+            if self.residual:       # x + ffn_down(a): the residual rides in the mat-vec epilogue as its bias operand
+                be.mul_mat(L["down"], self.a, out=self.res[li % 2], q8_in=self.q8a, bias=x[0])
+                x = self.res[li % 2]
+            else:
+                be.mul_mat(L["down"], self.a, out=self.x2, q8_in=self.q8a); self.allreduce(self.x2)
+                x = self.x2
+        self.hidden = x
         if with_head:
             be.mul_mat(self.head, x, out=self.logits)
 
@@ -250,6 +273,10 @@ class Model:
             # FUSED_UP_GATE (n > 8): up GEMM, gate GEMM with silu(gate)*up in its epilogue; it also emits the bf16 operand of ffn_down
             be.fused_up_gate(L["up"], L["gate"], self.h, "silu", out=self.a, x_bf16=self.hb, out_bf16=self.ab)
             be.mul_mat(L["down"], self.a, out=self.x2, x_bf16=self.ab)
+            if self.residual:
+                t.add(x, self.x2, out=self.res[li % 2])
+                x = self.res[li % 2]
+                continue
             if self.bf16_reduce:
                 last = li == len(self.layers) - 1
                 self.reducer.all_reduce_bf16(self.x2, out_bf16=self.xb, out_f32=self.x2 if last else None)    # f32 copy only where a mat-vec (head) reads it
@@ -257,45 +284,54 @@ class Model:
             else:
                 self.allreduce(self.x2)
             x = self.x2
+        self.hidden = x
         if with_head:
             be.mul_mat(self.head, x[-1:], out=self.logits)
 
 
-def bitnet_line(be, torch, steps, warmup, hbm_peak):
+def bitnet_line(be, torch, steps, warmup, hbm_peak, dump=None):
     """BASELINE.json configs[3] / SURVEY App. A config 4: bitnet-b1.58-3B (n_embd 3200, n_ff 8640, 26 layers), IQ2_BN (2.0 bpw + f32 row scale), the
     per-layer MUL_MAT nodes only (the output matrix of that model is not IQ2_BN).  K = 3200 / 8640 are not multiples of 256: decode takes the TMA ring
-    through the byte-granular geometry, prefill the int8 tensor-core path (ternary x int8 activations, tcgen05 kind::i8)."""
+    through the byte-granular geometry, prefill the int8 tensor-core path (ternary x int8 activations, wgmma u8 x s8)."""
     E, FF, NL, T = 3200, 8640, 26, 135
     gen = torch.Generator(device="cuda"); gen.manual_seed(4321)
-    def mk(m, k):
+    def mk(m, k, scale=1.0):
         rows = torch.randint(0, 256, (m, 4 + (k // 64) * 16), dtype=torch.uint8, device="cuda", generator=gen)
-        rs = (torch.rand(m, device="cuda", generator=gen) * 0.6 + 0.7) / k ** 0.5 * (torch.randint(0, 2, (m,), device="cuda", generator=gen).float() * 2 - 1)
+        rs = (torch.rand(m, device="cuda", generator=gen) * 0.6 + 0.7) * scale / k ** 0.5 * (torch.randint(0, 2, (m,), device="cuda", generator=gen).float() * 2 - 1)
         rows[:, 0:4] = rs.view(torch.uint8).view(m, 4)
         return be.set_tensor(T, rows.view(-1), m, k)
-    layers = [dict(wq=mk(E, E), wk=mk(E, E), wv=mk(E, E), wo=mk(E, E), up=mk(FF, E), gate=mk(FF, E), down=mk(E, FF)) for _ in range(NL)]
+    # residual stream as in Model; the random 2-bit codes have a larger gain than the IQ4_NL blocks, hence the smaller ffn_down scale
+    layers = [dict(wq=mk(E, E), wk=mk(E, E), wv=mk(E, E), wo=mk(E, E), up=mk(FF, E), gate=mk(FF, E), down=mk(E, FF, 0.04)) for _ in range(NL)]
     wbytes = sum(t.nbytes_wire for L in layers for t in L.values())
     f = lambda *sh: torch.empty(sh, dtype=torch.float32, device="cuda")
     out = {"workload": "bitnet-b1.58-3B IQ2_BN (BASELINE.json configs[3]): the 26 layers' MUL_MAT / FUSED_UP_GATE nodes in graph order, no output matrix",
            "algorithmic_bytes_per_step": wbytes}
     for n in (1, 512):
         x, q, k_, v, h, a, x2 = f(n, E), f(n, E), f(n, E), f(n, E), f(n, E), f(n, FF), f(n, E)
+        res = (f(n, E), f(n, E))
         x.normal_()
         def step():
             cur = x
-            for L in layers:
+            for i, L in enumerate(layers):
                 be.mul_mat_multi([L["wq"], L["wk"], L["wv"]], cur, [q, k_, v])
                 be.mul_mat(L["wo"], q, out=h)
                 be.fused_up_gate(L["up"], L["gate"], h, "silu", out=a)
-                be.mul_mat(L["down"], a, out=x2)
-                cur = x2
-        ms = time_graph(torch, step, steps if n == 1 else max(3, min(steps, 10)), warmup)
+                if n == 1:
+                    be.mul_mat(L["down"], a, out=res[i % 2], bias=cur[0])
+                else:
+                    be.mul_mat(L["down"], a, out=x2)
+                    torch.add(cur, x2, out=res[i % 2])
+                cur = res[i % 2]
+        ms = time_graph(torch, step, steps, warmup)
+        if dump:
+            dump(f"bitnet_{'tg' if n == 1 else 'pp512'}_hidden", res[(NL - 1) % 2])
         if n == 1:
             ach = wbytes / (ms * 1e-3) / 1e9
             out["tg"] = {"value": 1000.0 / ms, "unit": "tok/s", "ms_per_step": ms, "launches_per_step": 4 * NL,
                          "roofline": {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak}}
         else:
             ops = 2.0 * sum(t.m * t.k for L in layers for t in L.values()) * n
-            out["pp512"] = {"value": n * 1000.0 / ms, "unit": "tok/s", "ms_per_step": ms, "dtype": "u8 (ternary) x s8 activations -> s32 (tcgen05 kind::i8), f32 rescale",
+            out["pp512"] = {"value": n * 1000.0 / ms, "unit": "tok/s", "ms_per_step": ms, "dtype": "u8 (ternary) x s8 activations -> s32 (wgmma), f32 rescale",
                             "achieved_int8_TOP/s": ops / (ms * 1e-3) / 1e12}
     return out
 
@@ -344,6 +380,13 @@ def tp_correctness_gate(be, torch, dist, model, rank, world, n, n_check_layers=2
     model.layers = saved
     torch.cuda.empty_cache()
     return err, float(verdict.item()) == 0.0
+
+
+def make_dump(dirpath, rank=0, world=1):
+    """--dump-outputs: a writer name, tensor -> DIR/<name>[_rank<r>].npy (float32)."""
+    os.makedirs(dirpath, exist_ok=True)
+    suffix = f"_rank{rank}" if world > 1 else ""
+    return lambda name, t: np.save(os.path.join(dirpath, f"{name}{suffix}.npy"), t.detach().float().cpu().numpy())
 
 
 def time_graph(torch, fn, steps, warmup, dist=None, pre=None, post=None):
@@ -431,6 +474,7 @@ def main():
     ap.add_argument("--no-pp", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-mix", action="store_true", help="skip the default-quantisation-mix line (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step of every path as DIR/<name>.npy")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -475,6 +519,9 @@ def main():
         os.environ.setdefault("NCCL_DEBUG", "WARN")
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     torch.manual_seed(0)
+    dump = make_dump(args.dump_outputs, rank, world) if args.dump_outputs else None
+    if dump and world > 1 and rank == 0:
+        print("bench.py: the tensor-parallel model has no residual stream; its dumped outputs contract to zeros", file=sys.stderr)
 
     model = Model(be, torch, args.layers, tp=world, rank=rank)
     if model.fused_tp:
@@ -510,29 +557,25 @@ def main():
     ms_tg_e2e = time_graph(torch, model.step_tg, args.steps, args.warmup, dist,
                            pre=lambda: model.x.copy_(x_host, non_blocking=True),
                            post=lambda: (logits_host.copy_(model.logits, non_blocking=True), torch.cuda.current_stream().synchronize()))
+    if dump:
+        for k, v in model.outputs().items():
+            dump(f"tg_{k}", v)
     tok_s = 1000.0 / ms_tg
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    # the pp512 timed region is ~0.1 s at full SM clock: that is the BURST regime of MEASURED_PEAKS (its sustained figure was taken after 4 s at
-    # a 1410 MHz median); report against the burst peak and give the sustained fraction next to it
-    tf_peak = float(peaks.get("bf16_tflops", 1722.0))
-    tf_peak_sustained = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+    # without MEASURED_PEAKS.json: the H100 SXM data sheet (700 W card), HBM3 bandwidth and dense BF16 rate; a card with a lower power
+    # limit clocks down under sustained load, so expect a smaller share of these
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    tf_peak = float(peaks.get("bf16_tflops", 989.0))
+    tf_peak_sustained = float(peaks.get("bf16_tflops_sustained", tf_peak))
+    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (700 W)"
     bytes_tok = model.weight_bytes
-    traffic, traffic_src = {}, None
-    try:   # DRAM bytes per step measured by ncu --set full (scripts/make_traffic.py, committed under profiles/), N = 1 only
-        tf = [f for f in ("r2_traffic.json", "r1_traffic.json") if os.path.exists(os.path.join(ROOT, "profiles", f))]
-        traffic = json.load(open(os.path.join(ROOT, "profiles", tf[0]))) if tf and world == 1 and args.layers == N_LAYER else {}
-        traffic_src = f"static: profiles/{tf[0]} (ncu --set full capture of the same kernels, not measured in this run)" if traffic else None
-    except Exception:
-        pass
     ach = bytes_tok / (ms_tg * 1e-3) / 1e9
-    roof = {"bound": "hbm", "kernel": "k_mmvq<IQ4_NL>", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": traffic.get("tg", {}).get("dram_bytes_per_step"),
-            "traffic_source": traffic_src, "algorithmic_bytes_per_step": bytes_tok, "launches_per_step": model.launches_tg, "peak_source": peak_src,
+    roof = {"bound": "hbm", "kernel": "k_mmvq<IQ4_NL>", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": None,
+            "traffic_source": None, "algorithmic_bytes_per_step": bytes_tok, "launches_per_step": model.launches_tg, "peak_source": peak_src,
             "note": "the step consists only of k_mmvq launches; achieved = weight bytes per token / step time (per rank)"}
     line = {"metric": "llama-bench tg128 tok/s (MUL_MAT hot path)", "value": tok_s, "unit": "tok/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms_tg, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
@@ -545,18 +588,21 @@ def main():
         model.alloc(n)
         xh = torch.randn(n, N_EMBD).pin_memory()
         model.x.copy_(xh)
-        pp_steps = max(3, min(args.steps, 10))
+        pp_steps = args.steps
         ms_pp = time_graph(torch, model.step_pp, pp_steps, args.warmup, dist)
         ms_pp_e2e = time_graph(torch, model.step_pp, pp_steps, args.warmup, dist,
                                pre=lambda: model.x.copy_(xh, non_blocking=True),
                                post=lambda: (logits_host.copy_(model.logits, non_blocking=True), torch.cuda.current_stream().synchronize()))
+        if dump:
+            for k, v in model.outputs().items():
+                dump(f"pp512_{k}", v)
         fl = model_flops_pp(n, args.layers) / world
         tfs = fl / (ms_pp * 1e-3) / 1e12
         line["pp512"] = {"metric": "llama-bench pp512 tok/s (MUL_MAT hot path)", "value": n * 1000.0 / ms_pp, "unit": "tok/s", "ms_per_step": ms_pp, "steps": pp_steps,
-                         "dtype": "bf16 x bf16 -> f32 (tcgen05 kind::f16)", "e2e": {"value": n * 1000.0 / ms_pp_e2e, "unit": "tok/s", "h2d_bytes_per_step": n * N_EMBD * 4, "d2h_bytes_per_step": (N_VOCAB // world) * 4},
-                         "roofline": {"bound": "tensor", "kernel": "k_gemm_q<IQ4_NL> (fused dequant + tcgen05; + k_f32_to_bf16)", "achieved": tfs, "peak": tf_peak, "unit": "TFLOP/s", "frac": tfs / tf_peak,
-                                      "traffic": traffic.get("pp", {}).get("dram_bytes_per_step_gemm_only"), "traffic_source": traffic_src, "algorithmic_flops_per_step": fl,
-                                      "peak_source": peak_src + " burst (timed region << 1 s at max SM clock)", "frac_of_sustained_peak": tfs / tf_peak_sustained}}
+                         "dtype": "bf16 x bf16 -> f32 (wgmma)", "e2e": {"value": n * 1000.0 / ms_pp_e2e, "unit": "tok/s", "h2d_bytes_per_step": n * N_EMBD * 4, "d2h_bytes_per_step": (N_VOCAB // world) * 4},
+                         "roofline": {"bound": "tensor", "kernel": "k_gemm_q<IQ4_NL> (fused dequant + wgmma; + k_f32_to_bf16)", "achieved": tfs, "peak": tf_peak, "unit": "TFLOP/s", "frac": tfs / tf_peak,
+                                      "traffic": None, "traffic_source": None, "algorithmic_flops_per_step": fl,
+                                      "peak_source": peak_src, "frac_of_sustained_peak": tfs / tf_peak_sustained}}
     # ---------------- the default quantisation mix next to --pure (N = 1): IQ5_K attn_v, Q5_K ffn_down x4, Q6_K output ----------------
     if world == 1 and not args.no_mix and args.layers == N_LAYER:
         del model
@@ -564,6 +610,9 @@ def main():
         mm = Model(be, torch, args.layers, mix="default")
         mm.alloc(1); mm.x.copy_(x_host)
         ms_m = time_graph(torch, mm.step_tg, args.steps, args.warmup)
+        if dump:
+            for k, v in mm.outputs().items():
+                dump(f"default_mix_tg_{k}", v)
         ach_m = mm.weight_bytes / (ms_m * 1e-3) / 1e9
         mix = {"workload": "same model, default `llama-quantize ... IQ4_NL` mix (no --pure): attn_v IQ5_K, ffn_down of layers 0-3 Q5_K, output.weight Q6_K",
                "tg": {"value": 1000.0 / ms_m, "unit": "tok/s", "ms_per_step": ms_m, "launches_per_step": mm.launches_tg,
@@ -571,6 +620,9 @@ def main():
         if not args.no_pp:
             mm.alloc(512); mm.x.copy_(xh)
             ms_mp = time_graph(torch, mm.step_pp, pp_steps, args.warmup)
+            if dump:
+                for k, v in mm.outputs().items():
+                    dump(f"default_mix_pp512_{k}", v)
             tfm = model_flops_pp(512, args.layers) / (ms_mp * 1e-3) / 1e12
             mix["pp512"] = {"value": 512 * 1000.0 / ms_mp, "unit": "tok/s", "ms_per_step": ms_mp,
                             "roofline": {"bound": "tensor", "achieved": tfm, "peak": tf_peak, "unit": "TFLOP/s", "frac": tfm / tf_peak}}
@@ -578,7 +630,7 @@ def main():
         del mm
         torch.cuda.empty_cache()
         try:
-            line["bitnet"] = bitnet_line(be, torch, args.steps, args.warmup, hbm_peak)
+            line["bitnet"] = bitnet_line(be, torch, args.steps, args.warmup, hbm_peak, dump)
         except Exception as e:      # a side line must never cost the headline
             line["bitnet"] = {"error": repr(e)}
     # ---------------- cpu baseline (rank 0, N=1 only) ----------------

@@ -56,7 +56,7 @@ def plane_bytes(ggml_type: int, m: int, k: int) -> int:
 
 @dataclass
 class QuantTensor:
-    """A src0 of GGML_OP_MUL_MAT resident in HBM in the B200 plane layout (ne = [K, M] in ggml terms)."""
+    """A src0 of GGML_OP_MUL_MAT resident in HBM in the plane layout (ne = [K, M] in ggml terms)."""
     ggml_type: int
     m: int            # rows  (ne[1])
     k: int            # cols  (ne[0])
@@ -144,25 +144,31 @@ class Q8Scratch:
 
 
 def mul_mat(w: QuantTensor, x: torch.Tensor, out: torch.Tensor | None = None, x_bf16: torch.Tensor | None = None,
-            q8_in: "Q8Scratch | None" = None) -> torch.Tensor:
+            q8_in: "Q8Scratch | None" = None, bias: torch.Tensor | None = None) -> torch.Tensor:
     """GGML_OP_MUL_MAT: x f32 [N, K] -> dst f32 [N, M]  (ggml ne: src1 [K, N], dst [M, N]).
     x_bf16: optional result of convert_activations(x) (prefill only) to skip the per-call conversion.
-    q8_in: n = 1 only, x was produced by fused_up_gate(q8_out=q8_in): consume its already quantised image."""
+    q8_in: n = 1 only, x was produced by fused_up_gate(q8_out=q8_in): consume its already quantised image.
+    bias: f32 [M] added to every column in the mat-vec epilogue (the fused trailing GGML_OP_ADD); decode sizes (N <= 8) only."""
     _require_cuda()
     assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.shape[1] == w.k and x.stride(1) == 1
     n = x.shape[0]
+    if bias is not None:
+        if n > MMVQ_MAX_BATCH_SIZE:
+            raise ValueError("mul_mat: the bias operand exists for N <= 8 (mat-vec) only")
+        assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == w.m
+    bp = bias.data_ptr() if bias is not None else None
     dst = out if out is not None else torch.empty((n, w.m), dtype=torch.float32, device=x.device)
     L = _lib.lib()
     with torch.cuda.device(x.device):
         if n == 1 and q8_in is not None and q8_in.valid and q8_in.k == w.k:
-            check(L.b200q_mul_mat_vec_q8(w.ggml_type, w.ptr, x.data_ptr(), q8_in.buf.data_ptr(), dst.data_ptr(), w.m, w.k, None, _stream()), "b200q_mul_mat_vec_q8")
+            check(L.b200q_mul_mat_vec_q8(w.ggml_type, w.ptr, x.data_ptr(), q8_in.buf.data_ptr(), dst.data_ptr(), w.m, w.k, bp, _stream()), "b200q_mul_mat_vec_q8")
         elif n > MMVQ_MAX_BATCH_SIZE and x_bf16 is not None:
             assert x_bf16.dtype == torch.bfloat16 and x_bf16.shape == x.shape and x_bf16.is_contiguous()
             need = w.m * w.k * 2 + 256
             ws = _workspace(need, x.device)
             check(L.b200q_mul_mat_gemm_bf16(w.ggml_type, w.ptr, x_bf16.data_ptr(), dst.data_ptr(), w.m, w.k, n, ws.data_ptr(), ws.numel(), _stream()), "b200q_mul_mat_gemm_bf16")
         elif n <= MMVQ_MAX_BATCH_SIZE:
-            check(L.b200q_mul_mat_vec(w.ggml_type, w.ptr, x.data_ptr(), dst.data_ptr(), w.m, w.k, n, x.stride(0), None, _stream()), "b200q_mul_mat_vec")
+            check(L.b200q_mul_mat_vec(w.ggml_type, w.ptr, x.data_ptr(), dst.data_ptr(), w.m, w.k, n, x.stride(0), bp, _stream()), "b200q_mul_mat_vec")
         else:
             xc = x if x.is_contiguous() else x.contiguous()
             need = L.b200q_mul_mat_workspace(w.ggml_type, w.m, w.k, n)

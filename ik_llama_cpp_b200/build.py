@@ -1,4 +1,4 @@
-"""Build libb200q.so (sm_100a only) in-tree with nvcc.  `python -m ik_llama_cpp_b200.build [--force]`."""
+"""Build libb200q.so (sm_90a only) in-tree with nvcc.  `python -m ik_llama_cpp_b200.build [--force]`."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ LIB = os.path.join(HERE, "libb200q.so")
 OBJDIR = os.path.join(HERE, "_obj")
 SOURCES = ["b200q_decode_i0.cu", "b200q_decode_i1.cu", "b200q_decode_i2.cu", "b200q_decode_i3.cu", "b200q_wire.cu", "b200q_decode.cu", "b200q_gemm.cu", "b200q_reduce.cu", "b200q_api.cu"]
 HEADERS = ["b200q_types.cuh", "b200q_internal.h", "b200q_wire.cuh", "b200q_codebooks.h", "b200q_decode_common.cuh", "b200q_decode_ring.cuh", "b200q_decode_inst.inc", os.path.join("..", "..", "include", "b200q.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

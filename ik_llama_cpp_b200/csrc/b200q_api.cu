@@ -65,7 +65,7 @@ thread_local scratch g_x, g_y, g_ws, g_stage;
 int & opt_ring() { static int v = [] { const char * e = getenv("B200Q_RING"); return e ? atoi(e) : 1; }(); return v; }
 int & opt_fuse_epi() { static int v = [] { const char * e = getenv("B200Q_FUSE_EPILOGUE"); return e ? atoi(e) : 0; }(); return v; }
 int & opt_fused() { static int v = [] { const char * e = getenv("B200Q_FUSED_GEMM"); return e ? atoi(e) : 1; }(); return v; }
-// L2 warm-up of the next launch's weights: measured 753 vs 771 tok/s (slower: the prefetch competes with the running kernel's own stream) -> opt-in
+// L2 warm-up of the next launch's weights: measured slower (the prefetch competes with the running kernel's own stream) -> opt-in
 int & opt_pf() { static int v = [] { const char * e = getenv("B200Q_PREFETCH_NEXT"); return e ? atoi(e) : 0; }(); return v; }
 int & opt_q8() { static int v = [] { const char * e = getenv("B200Q_Q8_HANDOFF"); return e ? atoi(e) : 1; }(); return v; }
 int & opt_pdl() { static int v = [] { const char * e = getenv("B200Q_PDL"); return e ? atoi(e) : 1; }(); return v; }
@@ -250,8 +250,7 @@ int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const 
     if (comm) {
         d.tp.ll_mc = (float2 *)comm->ll_mc; d.tp.ll_local = (const float2 *)comm->ll_local; d.tp.ll_red = (float2 *)comm->ll_reduced; d.tp.ll_stride = comm->ll_stride;
         d.tp.world = comm->world_size; d.tp.rank = comm->rank; d.tp.seq = (uint32_t *)comm->ll_state; d.tp.in = reduce_in != 0; d.tp.out = reduce_out != 0;
-        // unicast variant (peer stores, rows of a CTA coalesced): measured SLOWER than the multicast stores at 2 GPUs (578-583 vs 626 tok/s, same box,
-        // profiles/r2_tp_timeline.md) -> opt-in only
+        // unicast variant (peer stores, rows of a CTA coalesced): measured slower than the multicast stores at 2 GPUs -> opt-in only
         static const int ucast = [] { const char * e = getenv("B200Q_TP_UNICAST"); return e ? atoi(e) : 0; }();
         if (ucast && comm->ll_peers && comm->world_size <= 8) {
             for (uint32_t r = 0; r < comm->world_size; ++r) {

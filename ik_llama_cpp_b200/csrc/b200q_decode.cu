@@ -1,9 +1,9 @@
-// b200q_decode.cu — HBM-bound kernels of the hot path for sm_100a:
+// b200q_decode.cu — HBM-bound kernels of the hot path for sm_90a:
 //   * k_repack / k_unrepack   wire (GGUF) blocks <-> plane layout (b200q_types.cuh), run once per tensor upload/download
 //   * k_mmvq                  decode mat-vec  dst[n][m] = sum_k W[m][k] x[n][k],  n <= 8   (replaces the reference's
 //                             quantize_q8_1 + mul_mat_vec_q / iqk_mul_mat_vec_q / fused_mul_mat_vec_q:
 //                             ggml/src/ggml-cuda/quantize.cu:13-47, mmvq-templates.cuh:68-330, iqk_mmvq_templates.cuh:21-300)
-//   * k_dequant_bf16          planes -> bf16 [M][K] (generic feeder of the tcgen05 GEMM for types without a fused prefill kernel)
+//   * k_dequant_bf16          planes -> bf16 [M][K] (generic feeder of the wgmma GEMM for types without a fused prefill kernel)
 //
 // Decode design (one launch per GGML_OP_MUL_MAT / FUSED_UP_GATE node, no tensor cores):
 //   - prologue: every CTA quantises the activation column(s) to q8_1 semantics straight into shared memory
@@ -93,7 +93,7 @@ int b200q_launch_repack(const void * wire, void * planes, const b200q_layout & L
 int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out, cudaStream_t st) {
     if (L.wire) return b200q_launch_wire_dequant_bf16(L.type, W, L.M, L.K, out, st);
     const int64_t total = L.M * (L.K / 32);
-    const int bs = 256; int64_t nb = (total + bs - 1) / bs; if (nb > 148 * 64) nb = 148 * 64; if (nb < 1) nb = 1;
+    const int bs = 256; int64_t nb = (total + bs - 1) / bs; if (nb > 132 * 64) nb = 132 * 64; if (nb < 1) nb = 1;
     switch (L.type) {
 #define X(T) case T: k_dequant_bf16<T><<<(unsigned)nb, bs, 0, st>>>((const uint8_t *)W, L, (__nv_bfloat16 *)out); break;
         B200Q_FOR_TYPES(X)

@@ -123,7 +123,7 @@ __device__ __forceinline__ void quantize_x_to_smem(const float * __restrict__ x,
             const int s_hi = __shfl_down_sync(0xffffffffu, s, 2);          // the second 16 of the 32-block
             if (valid) {
                 // natural order.  (Tried: two half planes [K/2 | K/2] so that the LDS.128 pairs of item_dot are conflict-free across the
-                // warp -> 659 vs 705 tok/s, slower; kept simple.)
+                // warp -> slower; kept simple.)
                 *reinterpret_cast<int2 *>(sq + (size_t)col * K + (size_t)ch * 8) = pk;
                 if ((ch & 3) == 0) {
                     sd[col * n32 + (ch >> 2)]  = __half2float(__float2half_rn(d));

@@ -16,8 +16,7 @@
 // decode mat-vec
 // ------------------------------------------------------------------------------------------------
 // L2 warm-up of the NEXT mat-vec's weights.  While this kernel runs, the next one cannot stream yet: its CTAs only become resident when ours leave
-// (shared memory), and then need a full HBM round trip for their first stages (measured: 3-4 us between the last warp of a short kernel and the first
-// useful instruction of the next).  The producer warp therefore issues cp.async.bulk.prefetch.L2 for exactly the bytes the next kernel's CTAs will
+// (shared memory), and then need a full HBM round trip for their first stages before the first useful instruction.  The producer warp therefore issues cp.async.bulk.prefetch.L2 for exactly the bytes the next kernel's CTAs will
 // request first; HBM works on them during OUR prologue / main loop, the next kernel's ring then fills from L2.
 //   mode 0: whole ranges ptr[q] .. +bytes[q], split evenly over this grid (small tensors: Q,K,V / wo)
 //   mode 1: plane q of a tensor whose units (rpu rows each, rowb[q] bytes per row) are split over `grid` CTAs like k_mmvq_ring does: the first
@@ -265,14 +264,14 @@ int launch_mmvq_id_type(const mmvq_id_args & a, bool upgate, int sm_count, bool 
 // into warp-private rings, decoupled from registers and from the data dependency on the previous kernel.
 //   * every warp owns S stages; a stage holds one SEGMENT (<= 128 items = 4096 weights) of one row of one tensor:
 //     one bulk copy per plane (rows are contiguous inside a plane), completion on a per-stage mbarrier (expect_tx);
-//   * lane 0 refills a stage as soon as the warp has consumed it, so W*S*stage bytes (~74 KB/SM) stay in flight —
-//     tools/membench.cu: 64 KB/SM of 2 KB bulk copies stream at 7.29 TB/s, LDG with 16 warps x 4 loads at 6.3 TB/s;
+//   * lane 0 refills a stage as soon as the warp has consumed it, so W*S*stage bytes (~74 KB/SM) stay in flight
+//     (tools/membench.cu compares bulk-copy rings with LDG streams at several depths);
 //   * the first S units of every warp are issued BEFORE griddepcontrol.wait: under programmatic dependent launch the
 //     next mat-vec of the graph is already resident (one 512-thread CTA per SM leaves room for a second) and has its
 //     ring full when the previous kernel finishes; only the activation quantisation is on the dependent path.
 // ------------------------------------------------------------------------------------------------
 #ifndef B200Q_SEG_ITEMS
-#define B200Q_SEG_ITEMS 128          // items (of 32 weights) per row per ring stage; tuning knob, see experiments/README.md
+#define B200Q_SEG_ITEMS 128          // items (of 32 weights) per row per ring stage; tuning knob (scripts/build_variant.sh)
 #endif
 #ifndef B200Q_MAX_STAGES
 #define B200Q_MAX_STAGES 4
@@ -376,14 +375,14 @@ __device__ __forceinline__ void issue_next_prefetch(const mmvq_pf & pf, int lane
 }
 
 // Warp 0 = producer (lane l streams the units of consumer warp l), warps 1..NCW = consumers.
-// A stage holds 2 x B200Q_SEG_ITEMS items (8192 weights) and is filled by ONE bulk copy per plane (tools/membench.cu `r`: the achieved HBM
-// bandwidth falls with the number of bulk copies in flight per SM: 6.0 TB/s with 4 copies per stage, 6.8 with 2, 7.0 with 1):
+// A stage holds 2 x B200Q_SEG_ITEMS items (8192 weights) and is filled by ONE bulk copy per plane (fewer, larger bulk copies in flight per SM
+// stream faster; tools/membench.cu measures it):
 //   PAIR = true  (K <= 4096, the row is one segment): a unit is a PAIR of adjacent output rows: inside every plane the two rows are adjacent, so they
 //                travel together; they share every activation load and all loop bookkeeping and give two independent dependency chains;
 //   PAIR = false (K > 4096, "long rows"): a unit is a segment of up to 256 items of ONE row (contiguous inside every plane); lane l owns items
 //                l + 32 i of both halves of the segment, the two halves are the two dependency chains.
 // TP: tensor-parallel instantiation (fused GGML_OP_REDUCE); a separate instantiation so that the single-GPU kernels carry none of it
-// (as runtime branches the extra code cost the plain path 4 %: 675 vs 705 tok/s)
+// (as runtime branches the extra code slowed the plain path down)
 // Q8: 0 = none, 1 = activations arrive as a b200q_q8 image (a.q8_in), 2 = fused up/gate also emits its result as one (a.q8_out)
 template <int TYPE, int NCOLS, bool UPGATE, bool MULTI, bool PAIR, bool TP, int Q8 = 0>
 __global__ void __launch_bounds__(32 * (B200Q_RING_CONSUMERS + 1), B200Q_MIN_CTAS) k_mmvq_ring(const mmvq_ring_args ra) {
@@ -667,7 +666,7 @@ __global__ void __launch_bounds__(32 * (B200Q_RING_CONSUMERS + 1), B200Q_MIN_CTA
         // q8 hand-off, producer side: once every consumer warp of this CTA has stored its rows (bar.sync: their stores are performed with respect to
         // the whole CTA), the CTA quantises the 32-row blocks of its static row range [RPU c0, RPU c1): blocks that lie inside the range directly,
         // the (at most two) blocks shared with a neighbouring CTA through an arrival counter: the CTA whose rows complete the block quantises it.
-        // One fence + atomic per SHARED block per CTA (round 2's first version paid a __threadfence per row pair: +4.6 us on the up/gate kernel).
+        // One fence + atomic per SHARED block per CTA (a __threadfence per row pair costs far more).
         asm volatile("bar.sync 1, %0;" ::"r"(cthreads) : "memory");
         const mmvq_seg & sgm = a.seg[0];
         const int M = (int)sgm.M, r0 = min(RPU * c0, M), r1 = min(RPU * c1, M);
@@ -875,8 +874,7 @@ static int launch_mmvq_ring_tp(const mmvq_args & a, const ring_geom & g0, int sm
     if (TP && a.tp.out && !MULTI) {
         // row buffer of a reduce_out launch: the rows of one CTA (a contiguous range, +-1 unit) are sent in one coalesced burst at the end
         const int64_t rows = (PAIR ? 2 : 1) * ((n_pairs + grid - 1) / grid + 1) + 2;
-        // (measured at 2 GPUs: 559 tok/s with the row buffer vs 575 without on the same box: no gain, the extra CTA barrier costs more than the
-        // coalescing saves -> off by default, B200Q_TP_ROWBUF=1 enables it)
+        // (measured at 2 GPUs: no gain, the extra CTA barrier costs more than the coalescing saves -> off by default, B200Q_TP_ROWBUF=1 enables it)
         static const int on_env = [] { const char * e = getenv("B200Q_TP_ROWBUF"); return e ? atoi(e) : -1; }();
         const bool on = on_env >= 0 ? on_env != 0 : a.tp.ll_peer[0] != nullptr;       // the coalescing only exists for the unicast stores
         if (on && rows <= 2048 && smem + rows * 4 + 16 <= budget) {

@@ -8,7 +8,7 @@
 //   (3) last CTA: multimem.red.add.u32 on the multicast flag (release.sys) -> every rank's flag += 1;
 //   (4) every CTA spins (ld.acquire.sys) until the local flag reaches world * use_count, then copies its slice of the
 //       local (now fully reduced) buffer to `out`.
-// tg: n = n_embd floats (16 KiB) -> 1 CTA, pure latency (~2 NVLink hops); pp512: 8 MiB -> up to 148 CTAs.
+// tg: n = n_embd floats (16 KiB) -> 1 CTA, pure latency (~2 NVLink hops); pp512: 8 MiB -> up to one CTA per SM (132).
 // f32 adds are performed by the switch in arrival order (like NCCL's NVLS algorithm): run-to-run LSB differences are possible.
 #include "b200q_internal.h"
 #include <cuda_runtime.h>

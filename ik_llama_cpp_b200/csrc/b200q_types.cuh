@@ -1,4 +1,4 @@
-// b200q_types.cuh — wire formats -> B200 device layout ("planes") -> canonical decode.
+// b200q_types.cuh — wire formats -> device layout ("planes") -> canonical decode.
 //
 // The wire format of every type is the reference's GGUF payload, consumed verbatim
 // (reference: ggml/src/ggml-common.h:166-775 block_* structs; value tables :2212-2250).
@@ -17,7 +17,7 @@
 // get_tensor / state save stay exact — same contract as the reference's run-time repack (-rtr).
 //
 // Canonical decode of one item (32 consecutive weights of one row), shared by the decode
-// mat-vec (b200q_mmvq.cu), the bf16 dequantiser and the tcgen05 prefill kernel (b200q_gemm.cu):
+// mat-vec (b200q_mmvq.cu), the bf16 dequantiser and the wgmma prefill kernel (b200q_gemm.cu):
 //
 //     w[e] = dl[e/16] * q[e] - ml[e/16],    q[e] = int8(va byte e) (+ int8(vb byte e) if HAS_B)
 //

@@ -1,7 +1,7 @@
 // b200q_wire.cu — kernels for the wire-layout types (b200q_wire.cuh): the types the reference's CUDA back-end serves through
 // vec_dot_<type>_q8_1 / iqk_mul_mat_vec_q (ggml-cuda/vecdotq.cuh:852-1127, iqk_mmvq.cu, template-instances/mmvq-instance-iq*_kt.cu,
 // -iq*_r4.cu) and through dequantize_block_* + GEMM for prefill (ggml-cuda/convert.cu, iqk_mmvq / mmq loaders mmq.cuh:2149-2445).
-//   * k_wire_dequant_bf16   wire bytes -> bf16 [M][K]: feeder of the tcgen05 GEMM (same path as the unfused plane types)
+//   * k_wire_dequant_bf16   wire bytes -> bf16 [M][K]: feeder of the wgmma GEMM (same path as the unfused plane types)
 //   * k_wire_mmvq           decode mat-vec, n <= 8: activations quantised to q8_1 in shared memory exactly like the plane kernels, one
 //                           warp per row, lanes stride the 32-weight items, f32 dot of the decoded weights with the q8 values:
 //                           the result is the quantity the reference's MMVQ kernels compute, up to f32 summation order.
@@ -215,7 +215,7 @@ int b200q_wire_check(int type, int64_t M, int64_t K) {
 int b200q_launch_wire_dequant_bf16(int type, const void * W, int64_t M, int64_t K, void * out, cudaStream_t st) {
     const int rc = b200q_wire_check(type, M, K); if (rc) return rc;
     const int64_t total = M * (K / 32);
-    const int bs = 128; int64_t nb = (total + bs - 1) / bs; if (nb > 148 * 64) nb = 148 * 64; if (nb < 1) nb = 1;
+    const int bs = 128; int64_t nb = (total + bs - 1) / bs; if (nb > 132 * 64) nb = 132 * 64; if (nb < 1) nb = 1;
     switch (type) {
 #define X(T) case T: k_wire_dequant_bf16<T><<<(unsigned)nb, bs, 0, st>>>((const uint8_t *)W, M, K, (__nv_bfloat16 *)out); break;
         B200Q_FOR_WIRE_TYPES(X)

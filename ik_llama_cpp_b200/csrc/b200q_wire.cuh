@@ -8,7 +8,7 @@
 //   row-interleaved x4    IQ2_K_R4 IQ3_K_R4 IQ4_K_R4 IQ5_K_R4 IQ4_KS_R4 IQ5_KS_R4 IQ1_S_R4 IQ1_M_R4   (iqk_quantize.cpp:7586, :7460, :6700, :6838, :5879, :6946, :8195, :8336)
 // One function per type family: b200q_wire_decode32<TYPE>(tensor base, K, row, it, w[32]) = weights 32*it .. 32*it+31 of `row` as f32,
 // bit-identical to the reference's to_float (checked against the oracle on the host: tests/test_host_emulation.py, and on the device).
-// The kernels that use it (b200q_wire.cu) are the generic feeders: a q8_1 mat-vec and the bf16 dequantiser of the tcgen05 GEMM.
+// The kernels that use it (b200q_wire.cu) are the generic feeders: a q8_1 mat-vec and the bf16 dequantiser of the wgmma GEMM.
 // Codebooks: b200q_codebooks.h, generated from values extracted by RUNNING the reference (tests/golden/gen_codebooks.py).
 #pragma once
 #include "b200q_types.cuh"

@@ -1,4 +1,4 @@
-/* b200q.h — C ABI of libb200q.so: the Blackwell (sm_100a) quantized mat-mul hot path of ik_llama.cpp.
+/* b200q.h — C ABI of libb200q.so: the Hopper (sm_90a) quantized mat-mul hot path of ik_llama.cpp.
  *
  * Plain C: pointers, sizes, ggml_type ids.  No torch / ggml types.  All device pointers are CUDA device
  * addresses on the current device; `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
@@ -82,7 +82,7 @@ B200Q_API int b200q_mul_mat_vec_q8(int type, const void * W, const float * x, co
  * The hint is consumed (cleared) by the next b200q_mul_mat_vec* / b200q_fused_up_gate_vec* call.  W_gate != NULL: fused up/gate (n_tensors = 1). */
 B200Q_API int b200q_decode_prefetch_next(int type, int n_tensors, const void * const * W, const void * W_gate, const int64_t * m, int64_t k);
 
-/* ---- prefill: tcgen05 GEMM ---- */
+/* ---- prefill: wgmma GEMM ---- */
 B200Q_API size_t b200q_mul_mat_workspace(int type, int64_t m, int64_t k, int64_t n);
 B200Q_API int b200q_mul_mat_gemm(int type, const void * W, const float * x, float * dst, int64_t m, int64_t k, int64_t n,
                        void * workspace, size_t workspace_bytes, void * stream);

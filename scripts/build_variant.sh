@@ -5,7 +5,7 @@ cd "$(dirname "$0")/.."
 name=$1; shift
 out=experiments/_variants; mkdir -p $out/obj_$name
 for f in b200q_decode_i0 b200q_decode_i1 b200q_decode_i2 b200q_decode_i3 b200q_decode b200q_gemm b200q_reduce b200q_api b200q_wire; do
-  /usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr "$@" \
+  /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr "$@" \
      -c ik_llama_cpp_b200/csrc/$f.cu -o $out/obj_$name/$f.o 2>/dev/null &
 done
 wait

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 ORACLE_ONLY_TYPES = []
-# plane layout (b200q_types.cuh: 16-byte low-bit plane per 32 weights, TMA-ring mat-vec, fused tcgen05 prefill for the 2-plane types)
+# plane layout (b200q_types.cuh: 16-byte low-bit plane per 32 weights, TMA-ring mat-vec, fused wgmma prefill for the 2-plane types)
 PLANE_TYPES = ["Q4_0", "Q4_1", "Q5_0", "Q5_1", "Q6_0", "Q8_0", "Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_NL", "IQ4_XS", "IQ2_K", "IQ3_K", "IQ4_K", "IQ5_K", "IQ4_KS", "IQ5_KS", "IQ2_KS", "IQ3_KS", "MXFP4", "IQ2_BN"]
 # wire layout (b200q_wire.cuh: GGUF bytes verbatim, generic decode): grid-codebook, trellis and row-interleaved types
 WIRE_TYPES = ["IQ2_XXS", "IQ2_XS", "IQ3_XXS", "IQ2_S", "IQ3_S", "IQ6_K", "IQ1_BN", "IQ4_KSS", "IQ1_S", "IQ1_M", "IQ2_KL", "IQ1_KT", "IQ2_KT", "IQ3_KT", "IQ4_KT",
@@ -19,7 +19,7 @@ ALL_TYPES = PLANE_TYPES + WIRE_TYPES      # every quantized type the reference's
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,10 +1,10 @@
 """Generate tests/golden/*.npz FROM THE UNMODIFIED REFERENCE (oracle/_ref, built by oracle/Makefile.ref).
 
-Run in the container that has /root/reference:   python tests/golden/gen_golden.py
+Run where oracle/_ref has been built from the reference sources:   python tests/golden/gen_golden.py
 For every supported wire type: seeded f32 weights -> ggml_quantize_chunk (reference) -> wire bytes;
 reference to_float(wire) -> dequantised f32; reference CPU backend MUL_MAT (IQK path) -> y_ref_cpu.
 The fixtures pin the oracle restatement (tests/test_oracle.py) and are replayed against the CUDA
-kernels on the GPU box (tests/test_gpu_parity.py), where /root/reference does not exist.
+kernels (tests/test_gpu_parity.py), so that the suite needs no reference build.
 """
 import os
 import sys
@@ -45,6 +45,52 @@ def main():
         np.savez_compressed(os.path.join(HERE, f"{name}.npz"), ggml_type=t, m=M, k=K, n=N, wire=wire, x=x,
                             dequant_ref=deq, y_ref_cpu=y_cpu, row_size=R.row_size(t, K))
         print(name, "wire", wire.size, "row_size", R.row_size(t, K))
+    if not only:
+        reference_live(R)
+
+
+# reference_live.npz: what tests/test_oracle.py::test_oracle_vs_live_reference and tests/test_gpu_parity.py::
+# test_fused_up_gate_limit_matches_reference_cpu_op compare against, recorded from the reference library so that the suite needs no
+# reference build.  Inputs are regenerated from the same seeds in the tests; to_float is stored as a SHA-256 of its f32 bytes where the
+# comparison is bit-exact, in full where it has a tolerance.
+LIVE_M, LIVE_K, LIVE_N = 8, 1024, 2
+LIVE_TOLERANT = ("IQ4_KS", "IQ5_KS", "IQ6_K")
+
+
+def live_inputs(name, t):
+    rng = np.random.default_rng(99 + t)
+    w = (rng.standard_normal((LIVE_M, LIVE_K)) * 0.05).astype(np.float32)
+    if name in ("IQ2_BN", "IQ1_BN"):
+        w = (rng.integers(-1, 2, (LIVE_M, LIVE_K)) * 0.37).astype(np.float32)
+    x = rng.uniform(-1, 1, (LIVE_N, LIVE_K)).astype(np.float32)
+    return w, x
+
+
+def reference_live(R):
+    import hashlib
+    sys.path.insert(0, os.path.dirname(HERE))
+    from conftest import make_wire
+    from oracle.oracle import Oracle
+    out = {}
+    for name in TYPES + WIRE_TYPES:
+        t = GGML_TYPE[name]
+        w, x = live_inputs(name, t)
+        wire = R.quantize(t, w)
+        deq = R.to_float(t, wire, LIVE_M, LIVE_K)
+        y, _ = R.mul_mat(t, wire, x, LIVE_M, n_threads=2)
+        out[f"{name}__wire"], out[f"{name}__row_size"], out[f"{name}__y_ref"] = wire, R.row_size(t, LIVE_K), y
+        if name in LIVE_TOLERANT:
+            out[f"{name}__to_float"] = deq
+        else:
+            out[f"{name}__to_float_sha256"] = np.frombuffer(hashlib.sha256(np.ascontiguousarray(deq, np.float32).tobytes()).digest(), np.uint8)
+    # GGML_OP_FUSED_UP_GATE (silu, op_params limit) through the reference CPU backend on the test's seeded Q4_0 tensors
+    O = Oracle()
+    m, k = 256, 512
+    wu, wg = make_wire(O, "Q4_0", m, k, seed=61), make_wire(O, "Q4_0", m, k, seed=62)
+    x = np.random.default_rng(9).standard_normal((1, k)).astype(np.float32) * 6
+    for limit in (0.0, 1.5):
+        out[f"fused_up_gate_silu_limit_{limit}"] = R.fused_up_gate(GGML_TYPE["Q4_0"], wu, wg, x, m, "silu", limit)
+    np.savez_compressed(os.path.join(HERE, "reference_live.npz"), **out)
 
 
 if __name__ == "__main__":

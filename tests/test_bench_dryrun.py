@@ -25,8 +25,9 @@ class _BE:
     def prefetch_next(self, ws, gate=None):
         assert all(hasattr(w, "m") for w in ws)
 
-    def mul_mat(self, w, x, out=None, x_bf16=None, q8_in=None):
+    def mul_mat(self, w, x, out=None, x_bf16=None, q8_in=None, bias=None):
         assert x.shape[1] == w.k and (out is None or out.shape[1] == w.m)
+        assert bias is None or (x.shape[0] == 1 and bias.shape == (w.m,))
         self.calls.append("mul_mat"); return out
 
     def mul_mat_multi(self, ws, x, outs=None, x_bf16=None):
@@ -46,7 +47,7 @@ def test_model_skeleton_walks_tg_and_pp(monkeypatch):
     monkeypatch.setattr(bench, "random_planes", lambda be, torch_, name, m, k, gen, scale: _T(m, k))
     gen = types.SimpleNamespace(manual_seed=lambda s: None)
     tt = types.SimpleNamespace(Generator=lambda device=None: gen, empty=lambda s, dtype=None, device=None: torch.empty(s, dtype=dtype),
-                               float32=torch.float32, bfloat16=torch.bfloat16)
+                               float32=torch.float32, bfloat16=torch.bfloat16, add=torch.add)
     be = _BE()
     m = bench.Model(be, tt, 2)
     m.alloc(1); m.step_tg()
@@ -64,3 +65,52 @@ def test_model_skeleton_walks_tg_and_pp(monkeypatch):
     assert be.calls.count("multi") == 2 and be.calls.count("mul_mat") == 7 and mm.launches_tg == 11
     assert mm.head.ggml_type == 14 and mm.layers[0]["down"].ggml_type == 13 and mm.layers[1]["wv"].ggml_type == 140
     mm.alloc(512); mm.step_pp()
+
+
+class _Reducer:
+    ok = True
+
+    def __init__(self, n):
+        self.buf = torch.zeros(n)
+
+    def reduced_view(self, n):
+        return self.buf[:n]
+
+    def all_reduce(self, t):
+        pass
+
+    def all_reduce_bf16(self, t, out_bf16=None, out_f32=None):
+        pass
+
+
+class _BE_TP(_BE):
+    NvlsReducer = _Reducer
+
+    def mul_mat_vec_tp(self, ws, x, outs, reducer, reduce_in=False, reduce_out=False, gate=None, unary=None):
+        assert (x is None) == reduce_in and (outs is None) == reduce_out
+        self.calls.append("tp")
+
+
+def test_tensor_parallel_walks_dump_their_outputs(monkeypatch, tmp_path):
+    """--gpus N: the fused-exchange decode walk (N = 2) and the separate-reduce walk (N = 4) both leave logits and a hidden state to dump."""
+    monkeypatch.setattr(bench, "random_planes", lambda be, torch_, name, m, k, gen, scale: _T(m, k))
+    for var in ("B200Q_TP_FUSED", "B200Q_NCCL_REDUCE", "B200Q_TP_BF16_REDUCE"):
+        monkeypatch.delenv(var, raising=False)
+    gen = types.SimpleNamespace(manual_seed=lambda s: None)
+    tt = types.SimpleNamespace(Generator=lambda device=None: gen, empty=lambda s, dtype=None, device=None: torch.empty(s, dtype=dtype),
+                               float32=torch.float32, bfloat16=torch.bfloat16, add=torch.add)
+    for tp, fused in ((2, True), (4, False)):
+        be = _BE_TP()
+        be.calls = []
+        m = bench.Model(be, tt, 2, tp=tp)
+        assert m.fused_tp == fused and not m.residual
+        dump = bench.make_dump(str(tmp_path / f"tp{tp}"), rank=1, world=tp)
+        m.alloc(1); m.step_tg()
+        assert be.calls.count("tp") == (9 if fused else 0)
+        for k, v in m.outputs().items():
+            dump(f"tg_{k}", v)
+        m.alloc(512); m.step_pp()
+        for k, v in m.outputs().items():
+            dump(f"pp512_{k}", v)
+        names = sorted(os.listdir(tmp_path / f"tp{tp}"))
+        assert names == ["pp512_hidden_rank1.npy", "pp512_logits_rank1.npy", "tg_hidden_rank1.npy", "tg_logits_rank1.npy"]

@@ -1,4 +1,4 @@
-"""Multi-GPU tests (need >= 2 B200s; skipped on a 1-GPU box): the in-tree NVLS all-reduce kernel vs the exact sum, eager and
+"""Multi-GPU tests (need >= 2 GPUs with NVLink multicast; skipped on a 1-GPU machine): the in-tree NVLS all-reduce kernel vs the exact sum, eager and
 replayed from a CUDA graph, and the row-parallel mat-vec + reduce against the unsharded oracle result."""
 import os
 import socket

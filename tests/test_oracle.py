@@ -1,4 +1,4 @@
-"""CPU tests: pin the oracle restatement to the reference (golden vectors + live reference library when present)."""
+"""CPU tests: pin the oracle restatement to the reference (golden vectors recorded from the unmodified reference library)."""
 import numpy as np
 import pytest
 
@@ -82,21 +82,23 @@ def test_half_conversions(oracle):
 
 
 @pytest.mark.parametrize("name", ALL_TYPES)
-def test_oracle_vs_live_reference(oracle, reflib, name):
-    """Live cross-check against the unmodified reference library (skipped where oracle/_ref is absent)."""
+def test_oracle_vs_live_reference(oracle, name):
+    """Cross-check against the unmodified reference library on a second data set: its quantiser's wire bytes, to_float and CPU MUL_MAT,
+    recorded in tests/golden/reference_live.npz by tests/golden/gen_golden.py (inputs regenerated here from the same seeds)."""
+    import hashlib
+    from golden.gen_golden import LIVE_M as m, LIVE_K as k, LIVE_TOLERANT, live_inputs
     t = GGML_TYPE[name]
-    rng = np.random.default_rng(99 + t)
-    m, k, n = 8, 1024, 2
-    w = (rng.standard_normal((m, k)) * 0.05).astype(np.float32)
-    if name in ("IQ2_BN", "IQ1_BN"):
-        w = (rng.integers(-1, 2, (m, k)) * 0.37).astype(np.float32)
-    wire = reflib.quantize(t, w)
-    assert reflib.row_size(t, k) == oracle.row_size(t, k)
-    a, b = oracle.dequantize(t, wire, m, k), reflib.to_float(t, wire, m, k)
-    _assert_dequant_equal(name, a, b)
-    x = rng.uniform(-1, 1, (n, k)).astype(np.float32)
-    y_ref, _ = reflib.mul_mat(t, wire, x, m, n_threads=2)
-    assert nmse(y_ref, oracle.mul_mat_exact(t, wire, x, m)) <= (1e-1 if name in REF_CPU_DEVIATES else 5e-4)
+    g = load_golden("reference_live")
+    _, x = live_inputs(name, t)
+    wire = g[f"{name}__wire"]
+    assert int(g[f"{name}__row_size"]) == oracle.row_size(t, k)
+    a = oracle.dequantize(t, wire, m, k)
+    if name in LIVE_TOLERANT:
+        _assert_dequant_equal(name, a, g[f"{name}__to_float"])
+    else:
+        assert hashlib.sha256(np.ascontiguousarray(a, np.float32).tobytes()).digest() == g[f"{name}__to_float_sha256"].tobytes(), \
+            f"{name}: dequantize != reference to_float (bit-exact expected)"
+    assert nmse(g[f"{name}__y_ref"], oracle.mul_mat_exact(t, wire, x, m)) <= (1e-1 if name in REF_CPU_DEVIATES else 5e-4)
 
 
 @pytest.mark.parametrize("name", ORACLE_ONLY_TYPES)

@@ -1,5 +1,5 @@
 // tools/membench.cu — calibration micro-benchmarks for the decode kernel design (not part of the product):
-// how many bytes in flight per SM does a B200 need to stream weights at HBM speed, via LDG.128 vs cp.async.bulk rings?
+// how many bytes in flight per SM does an H100 need to stream weights at HBM speed, via LDG.128 vs cp.async.bulk rings?
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -114,8 +114,8 @@ int main(int argc, char ** argv) {
             float ms = 0;
             for (int rep = 0; rep < 4; ++rep) {
                 if (rep == 1) cudaEventRecord(e0);
-                if (S == 2) { cudaFuncSetAttribute(k_bulk_multi<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); k_bulk_multi<2><<<296, (W + 1) * 32 - 32, sm>>>(d, nbytes, cs.c, out); }
-                else        { cudaFuncSetAttribute(k_bulk_multi<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); k_bulk_multi<3><<<296, (W + 1) * 32 - 32, sm>>>(d, nbytes, cs.c, out); }
+                if (S == 2) { cudaFuncSetAttribute(k_bulk_multi<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); k_bulk_multi<2><<<264, (W + 1) * 32 - 32, sm>>>(d, nbytes, cs.c, out); }
+                else        { cudaFuncSetAttribute(k_bulk_multi<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); k_bulk_multi<3><<<264, (W + 1) * 32 - 32, sm>>>(d, nbytes, cs.c, out); }
             }
             cudaEventRecord(e1); CK(cudaDeviceSynchronize()); cudaEventElapsedTime(&ms, e0, e1);
             printf("%-48s W=%2d x2 CTA S=%d  copies in flight/SM %3d  bytes in flight/SM %6.1f KB : %8.1f GB/s\n", cs.name, W, S, 2 * W * S * cs.c.nc, 2.0 * W * S * stage / 1024, nbytes / (ms / 3) / 1e6);
@@ -128,26 +128,26 @@ int main(int argc, char ** argv) {
     auto report = [&](const char * name, float ms, size_t bytes) { printf("%-44s %8.3f ms  %8.1f GB/s\n", name, ms, bytes / ms / 1e6); };
 #define RUN(name, bytes, ...) { __VA_ARGS__; CK(cudaDeviceSynchronize()); cudaEventRecord(e0); for (int r = 0; r < 3; ++r) { __VA_ARGS__; } cudaEventRecord(e1); CK(cudaDeviceSynchronize()); float ms; cudaEventElapsedTime(&ms, e0, e1); report(name, ms / 3, bytes); }
     const size_t n16 = nbytes / 16;
-    RUN("ldg U=1 148x1024", nbytes, (k_ldg<1><<<148, 1024>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=2 148x1024", nbytes, (k_ldg<2><<<148, 1024>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=4 148x1024", nbytes, (k_ldg<4><<<148, 1024>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=8 148x1024", nbytes, (k_ldg<8><<<148, 1024>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=4 148x512", nbytes, (k_ldg<4><<<148, 512>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=8 148x512", nbytes, (k_ldg<8><<<148, 512>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=4 296x512", nbytes, (k_ldg<4><<<296, 512>>>((const uint4 *)d, n16, out)));
-    RUN("ldg U=4 592x512 (4 CTA/SM x 16 warps)", nbytes, (k_ldg<4><<<592, 512>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=1 132x1024", nbytes, (k_ldg<1><<<132, 1024>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=2 132x1024", nbytes, (k_ldg<2><<<132, 1024>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=4 132x1024", nbytes, (k_ldg<4><<<132, 1024>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=8 132x1024", nbytes, (k_ldg<8><<<132, 1024>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=4 132x512", nbytes, (k_ldg<4><<<132, 512>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=8 132x512", nbytes, (k_ldg<8><<<132, 512>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=4 264x512", nbytes, (k_ldg<4><<<264, 512>>>((const uint4 *)d, n16, out)));
+    RUN("ldg U=4 528x512 (4 CTA/SM x 16 warps)", nbytes, (k_ldg<4><<<528, 512>>>((const uint4 *)d, n16, out)));
     // small problem sizes (one matrix): latency-dominated
     for (size_t mb : {9, 33, 66, 295}) {
-        char nm[64]; snprintf(nm, 64, "ldg U=4 296x512 %zu MB", mb);
-        RUN(nm, mb << 20, (k_ldg<4><<<296, 512>>>((const uint4 *)d, (mb << 20) / 16, out)));
-        snprintf(nm, 64, "ldg U=8 148x1024 %zu MB", mb);
-        RUN(nm, mb << 20, (k_ldg<8><<<148, 1024>>>((const uint4 *)d, (mb << 20) / 16, out)));
+        char nm[64]; snprintf(nm, 64, "ldg U=4 264x512 %zu MB", mb);
+        RUN(nm, mb << 20, (k_ldg<4><<<264, 512>>>((const uint4 *)d, (mb << 20) / 16, out)));
+        snprintf(nm, 64, "ldg U=8 132x1024 %zu MB", mb);
+        RUN(nm, mb << 20, (k_ldg<8><<<132, 1024>>>((const uint4 *)d, (mb << 20) / 16, out)));
     }
-#define BULK(S, CH, W) { size_t sm = (size_t)W * S * CH + W * S * 8 + 64; cudaFuncSetAttribute(k_bulk<S, CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); char nm[64]; snprintf(nm, 64, "bulk S=%d CH=%d W=%d (%zu KB/SM)", S, CH, W, sm / 1024); RUN(nm, nbytes, (k_bulk<S, CH><<<148, W * 32, sm>>>(d, nbytes, out))); }
+#define BULK(S, CH, W) { size_t sm = (size_t)W * S * CH + W * S * 8 + 64; cudaFuncSetAttribute(k_bulk<S, CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); char nm[64]; snprintf(nm, 64, "bulk S=%d CH=%d W=%d (%zu KB/SM)", S, CH, W, sm / 1024); RUN(nm, nbytes, (k_bulk<S, CH><<<132, W * 32, sm>>>(d, nbytes, out))); }
     BULK(2, 2048, 8) BULK(4, 2048, 8) BULK(4, 2048, 16) BULK(6, 2048, 16) BULK(2, 8192, 8) BULK(3, 8192, 8) BULK(2, 4096, 16) BULK(3, 4096, 16) BULK(8, 1024, 16)
     for (size_t mb : {9, 33, 66}) {
         size_t sm = (size_t)16 * 4 * 2048 + 16 * 4 * 8 + 64; char nm[64]; snprintf(nm, 64, "bulk S=4 CH=2048 W=16 %zu MB", mb);
-        RUN(nm, mb << 20, (k_bulk<4, 2048><<<148, 512, sm>>>(d, mb << 20, out)));
+        RUN(nm, mb << 20, (k_bulk<4, 2048><<<132, 512, sm>>>(d, mb << 20, out)));
     }
     return 0;
 }

@@ -291,6 +291,54 @@ def mul_mat_id(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "Exper
     return dst
 
 
+def _mul_mat_id_args(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "ExpertTensor | None"):
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.is_contiguous() and x.shape[2] == w.k
+    assert ids.is_cuda and ids.dtype == torch.int32 and ids.dim() == 2 and ids.is_contiguous() and ids.shape[0] == x.shape[0]
+    if gate is not None:
+        assert gate.ggml_type == w.ggml_type and (gate.n_expert, gate.m, gate.k) == (w.n_expert, w.m, w.k)
+    n_tokens, nb1, n_used = x.shape[0], x.shape[1], ids.shape[1]
+    assert n_used % nb1 == 0
+    return n_tokens, nb1, n_used
+
+
+def mul_mat_id_workspace(w: ExpertTensor, n_tokens: int, n_used: int, nb1: int, up_gate: bool) -> int:
+    """Bytes of device workspace the grouped MoE GEMM needs; 0 exactly when mul_mat_id_dispatch takes the mat-vec path."""
+    return int(_lib.lib().b200q_mul_mat_id_workspace(w.ggml_type, w.m, w.k, n_used, nb1, n_tokens, w.n_expert, int(up_gate)))
+
+
+def mul_mat_id_gemm(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "ExpertTensor | None" = None, unary: str = "silu", limit: float = 0.0,
+                    out: torch.Tensor | None = None) -> torch.Tensor:
+    """GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE on the grouped tensor-core GEMM over expert-sorted slots (prefill), whatever the batch.
+    Same operands and result as mul_mat_id, except that ids outside [0, n_expert) give zero rows.  Routing stays on the device."""
+    _require_cuda()
+    n_tokens, nb1, n_used = _mul_mat_id_args(w, x, ids, gate)
+    dst = out if out is not None else torch.empty((n_tokens, n_used, w.m), dtype=torch.float32, device=x.device)
+    L = _lib.lib()
+    # the workspace query returns 0 below the dispatch threshold: size it from a batch above it (the layout only grows with the batch)
+    need = mul_mat_id_workspace(w, max(n_tokens, 8 * w.n_expert // n_used + 1), n_used, nb1, gate is not None)
+    ws = _workspace(need, x.device)
+    with torch.cuda.device(x.device):
+        check(L.b200q_mul_mat_id_gemm(w.ggml_type, w.ptr, gate.ptr if gate is not None else None, w.n_expert, ids.data_ptr(), x.data_ptr(), dst.data_ptr(),
+                                      w.m, w.k, n_used, nb1, n_tokens, UNARY[unary], float(limit), ws.data_ptr(), ws.numel(), _stream()), "b200q_mul_mat_id_gemm")
+    return dst
+
+
+def mul_mat_id_dispatch(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "ExpertTensor | None" = None, unary: str = "silu", limit: float = 0.0,
+                        out: torch.Tensor | None = None) -> torch.Tensor:
+    """What the GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE node runs (b200q_mul_mat_id): the grouped GEMM above the rows-per-expert threshold,
+    mul_mat_id's mat-vec kernel below it."""
+    _require_cuda()
+    n_tokens, nb1, n_used = _mul_mat_id_args(w, x, ids, gate)
+    dst = out if out is not None else torch.empty((n_tokens, n_used, w.m), dtype=torch.float32, device=x.device)
+    need = mul_mat_id_workspace(w, n_tokens, n_used, nb1, gate is not None)
+    ws = _workspace(need, x.device) if need else None
+    with torch.cuda.device(x.device):
+        check(_lib.lib().b200q_mul_mat_id(w.ggml_type, w.ptr, gate.ptr if gate is not None else None, w.n_expert, ids.data_ptr(), x.data_ptr(), dst.data_ptr(),
+                                          w.m, w.k, n_used, nb1, n_tokens, UNARY[unary], float(limit), ws.data_ptr() if ws is not None else None,
+                                          ws.numel() if ws is not None else 0, _stream()), "b200q_mul_mat_id")
+    return dst
+
+
 def dequantize_bf16(w: QuantTensor) -> torch.Tensor:
     _require_cuda()
     out = torch.empty((w.m, w.k), dtype=torch.bfloat16, device=w.planes.device)

@@ -402,7 +402,7 @@ int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_ex
     if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_mul_mat_id_vec: activations must be 16-byte aligned");
     if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_vec: bad token / slot counts");
     // the quantised activation columns of a launch live in shared memory: larger batches are walked in token chunks (same kernel, the expert ids
-    // never leave the device).  This is the functional path for MoE prefill, not a tuned one: a grouped tensor-core GEMM is not built.
+    // never leave the device).  Prefill batches are served by the grouped GEMM (b200q_mul_mat_id_gemm) once b200q_mul_mat_id selects it.
     const int64_t col_bytes = (int64_t)nb1 * (k + k / 4);
     int chunk = (int)((200 * 1024) / (col_bytes > 0 ? col_bytes : 1));
     static const int forced = [] { const char * e = getenv("B200Q_MOE_CHUNK_TOKENS"); return e ? atoi(e) : 0; }();
@@ -418,6 +418,40 @@ int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_ex
         if (rc) return rc;
     }
     return B200Q_OK;
+}
+
+/* MoE prefill: grouped wgmma GEMM over expert-sorted slots (b200q_moe.cu), versus the mat-vec kernel, which needs no routing or gather pass.
+ * Crossovers measured with scripts/bench_moe.py on an H100 80GB HBM3 at 700 W, 1-256 tokens (Qwen3-30B-A3B Q4_K / IQ4_K, Mixtral-8x7B IQ4_NL,
+ * DeepSeek-V3 TP-8 shard IQ2_XXS; DESIGN.md §4):
+ *  - MOE_FUSED_UP_GATE follows the average rows per expert, n_slots / n_expert: at 4 rows Mixtral is still 0.82x while the others are 1.3-1.45x,
+ *    at 6 rows every shape is 1.4-2.2x faster on the grouped path.  Grouped when n_slots > 5 * n_expert.
+ *  - MUL_MAT_ID follows the number of slots, whatever the expert count: 24 slots 0.84x (Mixtral), 32 slots 0.94-1.08x, 64 slots 1.18-2.3x on
+ *    every shape.  Grouped when n_slots > 32. */
+static constexpr int64_t MOE_UP_GATE_MIN_ROWS_PER_EXPERT = 5;
+static constexpr int64_t MOE_MUL_MAT_ID_MIN_SLOTS = 32;
+size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate) {
+    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate)) return 0;
+    const int64_t n_slots = (int64_t)n_tokens * n_used;
+    if (up_gate ? n_slots <= MOE_UP_GATE_MIN_ROWS_PER_EXPERT * n_expert : n_slots <= MOE_MUL_MAT_ID_MIN_SLOTS) return 0;
+    return b200q_moe_gemm_workspace_bytes(type, m, k, n_slots, n_expert, up_gate);
+}
+int b200q_mul_mat_id_gemm(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
+                          int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
+    if (!W || !ids || !x || !dst || !workspace || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_gemm: bad argument");
+    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_id_gemm: no CUDA device");
+    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_gemm: bad token / slot counts");
+    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, W_gate != nullptr))
+        return fail(B200Q_E_SHAPE, "b200q_mul_mat_id_gemm: shape not supported by the grouped GEMM (K %% 256, n_expert <= 1024, type)");
+    b200q_mmvq_id_desc d; memset(&d, 0, sizeof d);
+    d.type = type; d.W = W; d.W2 = W_gate; d.ids = ids; d.x = x; d.dst = dst; d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.n_tokens = n_tokens;
+    d.act = unary; d.limit = limit; d.sm_count = di.sm_count;
+    return check_launch(b200q_launch_moe_gemm(d, workspace, workspace_bytes, (cudaStream_t)stream), "b200q_mul_mat_id_gemm");
+}
+int b200q_mul_mat_id(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
+                     int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
+    if (b200q_mul_mat_id_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, W_gate != nullptr) == 0)
+        return b200q_mul_mat_id_vec(type, W, W_gate, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, stream);
+    return b200q_mul_mat_id_gemm(type, W, W_gate, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, workspace, workspace_bytes, stream);
 }
 int b200q_mul_mat_host(int type, const void * W, const float * x_host, float * dst_host, int64_t m, int64_t k, int64_t n, void * stream) {
     cudaStream_t st = (cudaStream_t)stream; cudaError_t e; int rc;

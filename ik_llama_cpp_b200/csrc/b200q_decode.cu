@@ -37,10 +37,14 @@ __global__ void k_repack(const uint8_t * __restrict__ wire, uint8_t * __restrict
 }
 
 // ------------------------------------------------------------------------------------------------
-// dequantise planes -> bf16 [M][K]
+// dequantise planes -> bf16 [M][K]; blockIdx.y = expert e0 + y of an expert tensor (experts L.total_bytes apart) -> out[y][M][K],
+// skipped when `bounds` says that it received no rows (MoE prefill)
 // ------------------------------------------------------------------------------------------------
 template <int TYPE>
-__global__ void k_dequant_bf16(const uint8_t * __restrict__ W, b200q_layout L, __nv_bfloat16 * __restrict__ out) {
+__global__ void k_dequant_bf16(const uint8_t * __restrict__ W, b200q_layout L, __nv_bfloat16 * __restrict__ out, int e0, const int * __restrict__ bounds) {
+    const int e = e0 + (int)blockIdx.y;
+    if (bounds != nullptr && __ldg(bounds + e + 1) == __ldg(bounds + e)) return;
+    W += (int64_t)e * L.total_bytes; out += (int64_t)blockIdx.y * L.M * L.K;
     const int64_t n32 = L.K / 32, total = L.M * n32;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t row = i / n32, it = i % n32;
@@ -91,11 +95,16 @@ int b200q_launch_repack(const void * wire, void * planes, const b200q_layout & L
 }
 
 int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out, cudaStream_t st) {
-    if (L.wire) return b200q_launch_wire_dequant_bf16(L.type, W, L.M, L.K, out, st);
+    return b200q_launch_dequant_bf16_experts(W, L, out, 0, 1, nullptr, st);
+}
+int b200q_launch_dequant_bf16_experts(const void * W, const b200q_layout & L, void * out, int e0, int n_e, const int * bounds, cudaStream_t st) {
+    if (n_e < 1 || n_e > 65535) return -2;
+    if (L.wire) return b200q_launch_wire_dequant_bf16_experts(L.type, W, L.M, L.K, L.total_bytes, out, e0, n_e, bounds, st);
     const int64_t total = L.M * (L.K / 32);
-    const int bs = 256; int64_t nb = (total + bs - 1) / bs; if (nb > 132 * 64) nb = 132 * 64; if (nb < 1) nb = 1;
+    const int bs = 256; int64_t nb = (total + bs - 1) / bs; const int64_t cap = 132 * 64 / n_e > 1 ? 132 * 64 / n_e : 1; if (nb > cap) nb = cap; if (nb < 1) nb = 1;
+    const dim3 grid((unsigned)nb, (unsigned)n_e);
     switch (L.type) {
-#define X(T) case T: k_dequant_bf16<T><<<(unsigned)nb, bs, 0, st>>>((const uint8_t *)W, L, (__nv_bfloat16 *)out); break;
+#define X(T) case T: k_dequant_bf16<T><<<grid, bs, 0, st>>>((const uint8_t *)W, L, (__nv_bfloat16 *)out, e0, bounds); break;
         B200Q_FOR_TYPES(X)
 #undef X
         default: return -1;

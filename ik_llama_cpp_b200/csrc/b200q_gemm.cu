@@ -15,6 +15,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <climits>
 #include <cstdlib>
 #include <cstring>
@@ -57,6 +58,11 @@ __device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0,
 __device__ __forceinline__ void tma_load_2d(void * smem_dst, const CUtensorMap * tm, uint64_t * bar, int x, int y) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(x), "r"(y) : "memory");
+}
+// 3-D map (bytes or elements along the row, row, matrix): one map covers all experts of a MoE weight tensor
+__device__ __forceinline__ void tma_load_3d(void * smem_dst, const CUtensorMap * tm, uint64_t * bar, int x, int y, int z) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+                 ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap * tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)tm) : "memory");
@@ -211,10 +217,22 @@ template <int BN> struct gemm_cfg {
     static_assert(SMEM <= 227 * 1024, "k_gemm_bf16: shared memory");
 };
 
-template <int BN>
+// MoE prefill (GROUPED): blockIdx.y indexes the tile table of the expert-sorted activation rows (k_moe_route); a tile covers the rows
+// [n0, n0 + BN) of ONE expert e, the columns at or past bounds[e + 1] belong to the next expert and are dropped in the epilogue, which stores
+// each kept column straight to its slot: dst[slot[n]][m].  CTAs past the device-side tile count return at once.
+__device__ __forceinline__ bool moe_tile(const b200q_moe_route & rt, int & e, int & n0, int & n_end) {
+    const int tile = __ldg(rt.tile_start + rt.e0) + (int)blockIdx.y;
+    if (tile >= __ldg(rt.tile_start + rt.e1)) return false;
+    const int2 te = __ldg(rt.tiles + tile);
+    e = te.x; n0 = te.y; n_end = __ldg(rt.bounds + e + 1);
+    return true;
+}
+
+// GROUPED: A is the bf16 scratch of experts e0 .. e1-1 through a 3-D map (k, row, expert - e0)
+template <int BN, bool GROUPED = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_gemm_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            float * __restrict__ dst, int M, int N, int K, int k_split) {
+            float * __restrict__ dst, int M, int N, int K, int k_split, const b200q_moe_route rt) {
     using cfg = gemm_cfg<BN>;
     extern __shared__ unsigned char smem_raw[];
     unsigned char * smem = reinterpret_cast<unsigned char *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -222,7 +240,9 @@ k_gemm_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     uint64_t * empty_bar = full_bar + cfg::STAGES;
 
     const int warp = warp_uniform_id(), lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+    const int m0 = blockIdx.x * BM;
+    int n0 = blockIdx.y * BN, e = 0, n_end = N;
+    if constexpr (GROUPED) { if (!moe_tile(rt, e, n0, n_end)) return; }
     const int nk_total = (K + BK - 1) / BK;
     const int nk_per = (nk_total + k_split - 1) / k_split;
     const int kb0 = blockIdx.z * nk_per;
@@ -243,7 +263,8 @@ k_gemm_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 mbar_wait(&empty_bar[s], ph ^ 1);
                 unsigned char * sa = smem + (size_t)s * cfg::STAGE_BYTES; unsigned char * sb = sa + cfg::A_BYTES;
                 mbar_expect_tx(&full_bar[s], cfg::STAGE_BYTES);
-                tma_load_2d(sa, &tmA, &full_bar[s], (kb0 + i) * BK, m0);
+                if constexpr (GROUPED) tma_load_3d(sa, &tmA, &full_bar[s], (kb0 + i) * BK, m0, e - rt.e0);
+                else tma_load_2d(sa, &tmA, &full_bar[s], (kb0 + i) * BK, m0);
                 tma_load_2d(sb, &tmB, &full_bar[s], (kb0 + i) * BK, n0);
             }
         }
@@ -274,7 +295,9 @@ k_gemm_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) {
         const int m = m0 + 64 * wg + acc_row(wl, lane, j), n = n0 + acc_col(lane, j);
-        if (m < M && n < N) {
+        if constexpr (GROUPED) {
+            if (m < M && n < n_end) dst[(size_t)__ldg(rt.slot + n) * M + m] = acc[j];
+        } else if (m < M && n < N) {
             float * p = dst + (size_t)n * M + m;
             if (k_split > 1) atomicAdd(p, acc[j]); else *p = acc[j];
         }
@@ -322,6 +345,7 @@ struct gemmq_args {
     CUtensorMap tmP0[GEMMQ_MAX_SEGS], tmP1[GEMMQ_MAX_SEGS], tmP2[GEMMQ_MAX_SEGS], tmB;
     gemmq_seg seg[GEMMQ_MAX_SEGS];
     int n_seg, N, K, k_split, act; float limit;
+    b200q_moe_route rt;                          // GROUPED only: the plane maps are 3-D (bytes along the row, row, expert)
 };
 
 // carry-less per-byte add of two packed int8x4 (the A/B halves of the sign-fill LUT)
@@ -335,7 +359,7 @@ template <int J> __device__ __forceinline__ float biased_byte_to_float(uint32_t 
     return __uint_as_float(bits) - 8388736.0f;
 }
 
-template <int TYPE, int NB>
+template <int TYPE, int NB, bool GROUPED = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_gemm_q(const __grid_constant__ gemmq_args a) {
     using cfg = gemmq_cfg<TYPE, NB>;
@@ -356,7 +380,9 @@ k_gemm_q(const __grid_constant__ gemmq_args a) {
     uint64_t * raw_full = b_empty + cfg::B_STAGES, * raw_empty = raw_full + cfg::RAW_STAGES;
 
     const int warp = warp_uniform_id(), lane = threadIdx.x & 31;
-    const int m0 = ((int)blockIdx.x - a.seg[sg].tile0) * BM, n0 = blockIdx.y * BN;
+    const int m0 = ((int)blockIdx.x - a.seg[sg].tile0) * BM;
+    int n0 = blockIdx.y * BN, e = 0, n_end = N;
+    if constexpr (GROUPED) { if (!moe_tile(a.rt, e, n0, n_end)) return; }
     // K is walked in raw blocks of 256 weights; split-K over blockIdx.z in units of raw blocks
     const int nr_total = (K + RAW_K - 1) / RAW_K;
     const int nr_per = (nr_total + k_split - 1) / k_split;
@@ -382,9 +408,15 @@ k_gemm_q(const __grid_constant__ gemmq_args a) {
                 mbar_wait(&raw_empty[rs], rph ^ 1);
                 unsigned char * raw = sR + (size_t)rs * cfg::RAW_BYTES;
                 mbar_expect_tx(&raw_full[rs], cfg::RAW_BYTES);
-                tma_load_2d(raw, tmP0, &raw_full[rs], (rb0 + r) * 128, m0);                // bytes along the row
-                tma_load_2d(raw + cfg::RAW_P0, tmP1, &raw_full[rs], (rb0 + r) * cfg::P1, m0);
-                if (cfg::P2) tma_load_2d(raw + cfg::RAW_P0 + cfg::RAW_P1, tmP2, &raw_full[rs], (rb0 + r) * cfg::P2, m0);
+                if constexpr (GROUPED) {
+                    tma_load_3d(raw, tmP0, &raw_full[rs], (rb0 + r) * 128, m0, e);
+                    tma_load_3d(raw + cfg::RAW_P0, tmP1, &raw_full[rs], (rb0 + r) * cfg::P1, m0, e);
+                    if (cfg::P2) tma_load_3d(raw + cfg::RAW_P0 + cfg::RAW_P1, tmP2, &raw_full[rs], (rb0 + r) * cfg::P2, m0, e);
+                } else {
+                    tma_load_2d(raw, tmP0, &raw_full[rs], (rb0 + r) * 128, m0);                // bytes along the row
+                    tma_load_2d(raw + cfg::RAW_P0, tmP1, &raw_full[rs], (rb0 + r) * cfg::P1, m0);
+                    if (cfg::P2) tma_load_2d(raw + cfg::RAW_P0 + cfg::RAW_P1, tmP2, &raw_full[rs], (rb0 + r) * cfg::P2, m0);
+                }
                 for (int q = 0; q < RAW_K / BK && ib < nk; ++q, ++ib) {
                     const int s = ib % cfg::B_STAGES; const uint32_t ph = (ib / cfg::B_STAGES) & 1;
                     mbar_wait(&b_empty[s], ph ^ 1);
@@ -459,7 +491,9 @@ k_gemm_q(const __grid_constant__ gemmq_args a) {
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) {
         const int m = m0 + 64 * wg + acc_row(wl, lane, j), n = n0 + acc_col(lane, j);
-        if (m < M && n < N) {
+        if constexpr (GROUPED) {
+            if (m < M && n < n_end) dst[(size_t)__ldg(a.rt.slot + n) * M + m] = acc[j];
+        } else if (m < M && n < N) {
             float * p = dst + (size_t)n * M + m;
             if (k_split > 1) { atomicAdd(p, acc[j]); continue; }
             float v = acc[j];
@@ -649,7 +683,10 @@ __global__ void k_mul_unary(const float * gate /* may alias dst: no __restrict__
 
 // f32 [N][K] (row stride xs) -> bf16 [N][K].  HBM-bound glue between the GEMMs (12 MB per 512 x 4096 activation): a thread converts 8 consecutive
 // values (two LDG.128 -> one STG.128) and keeps U such groups in flight, so that enough loads are outstanding to approach HBM bandwidth.
-__global__ void __launch_bounds__(256) k_f32_to_bf16(const float * __restrict__ x, int64_t xs, __nv_bfloat16 * __restrict__ out, int64_t K, int64_t N) {
+// MAP (MoE gather): output row n reads input row row_map[n]; a negative entry (past the routed rows) gives a zero row.
+template <bool MAP = false>
+__global__ void __launch_bounds__(256) k_f32_to_bf16(const float * __restrict__ x, int64_t xs, __nv_bfloat16 * __restrict__ out, int64_t K, int64_t N,
+                                                     const int * __restrict__ row_map = nullptr) {
     constexpr int U = 4;
     const int64_t k8 = K / 8, total8 = N * k8, stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < total8; i0 += U * stride) {
@@ -657,7 +694,12 @@ __global__ void __launch_bounds__(256) k_f32_to_bf16(const float * __restrict__ 
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const int64_t i = i0 + u * stride;
-            if (i < total8) { const int64_t n = i / k8, c = i % k8; const float4 * p = reinterpret_cast<const float4 *>(x + n * xs + 8 * c); a[u] = __ldg(p); b[u] = __ldg(p + 1); }
+            if (i < total8) {
+                const int64_t n = i / k8, c = i % k8;
+                const int64_t src = MAP ? (int64_t)__ldg(row_map + n) : n;
+                if (MAP && src < 0) { a[u] = b[u] = make_float4(0.f, 0.f, 0.f, 0.f); continue; }
+                const float4 * p = reinterpret_cast<const float4 *>(x + src * xs + 8 * c); a[u] = __ldg(p); b[u] = __ldg(p + 1);
+            }
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
@@ -722,7 +764,38 @@ int launch_gemm_bf16(const void * A_bf16, const void * B_bf16, float * dst, int6
         configured[dev] = true;
     }
     dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((N + BN - 1) / BN), (unsigned)k_split);
-    k_gemm_bf16<BN><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(tmA, tmB, dst, (int)M, (int)N, (int)K, k_split);
+    k_gemm_bf16<BN><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(tmA, tmB, dst, (int)M, (int)N, (int)K, k_split, b200q_moe_route{});
+    return (int)cudaGetLastError();
+}
+
+// experts of a bf16 scratch [n_mat][rows][cols], box = 64 cols x box_rows x 1 matrix, 128B swizzle
+int make_tmap_bf16_3d(CUtensorMap * tm, const void * ptr, int64_t rows, int64_t cols, int64_t n_mat, int box_rows) {
+    encode_tiled_fn enc = get_encode(); if (!enc) return -1;
+    cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)n_mat};
+    cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)(rows * cols * 2)};
+    cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(ptr), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? 0 : -2;
+}
+
+template <int BN>
+int launch_gemm_bf16_grouped(const void * A_bf16, int n_mat, const b200q_moe_gemm & g, float * dst, const b200q_moe_route & rt, cudaStream_t st) {
+    using cfg = gemm_cfg<BN>;
+    CUtensorMap tmA, tmB;
+    if (make_tmap_bf16_3d(&tmA, A_bf16, g.M, g.K, n_mat, BM)) return -10;
+    if (make_tmap_bf16(&tmB, g.xb, g.n_rows, g.K, BN)) return -11;
+    static bool configured[B200Q_MAX_DEVICES] = {};
+    const int dev = b200q_current_device();
+    if (!configured[dev]) {
+        if (cudaFuncSetAttribute(k_gemm_bf16<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg::SMEM) != cudaSuccess) return -12;
+        configured[dev] = true;
+    }
+    // upper bound of the tiles of experts e0 .. e1-1: every expert's last tile may be partial
+    const int64_t tiles = (g.n_rows + BN - 1) / BN + std::min<int64_t>(rt.e1 - rt.e0, g.n_rows);
+    dim3 grid((unsigned)((g.M + BM - 1) / BM), (unsigned)tiles, 1);
+    k_gemm_bf16<BN, true><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(tmA, tmB, dst, (int)g.M, (int)g.n_rows, (int)g.K, 1, rt);
     return (int)cudaGetLastError();
 }
 
@@ -771,6 +844,47 @@ int launch_gemm_q(const b200q_gemm_multi & d, int k_split, cudaStream_t st) {
     }
     dim3 grid((unsigned)tiles, (unsigned)((d.N + cfg::BN - 1) / cfg::BN), (unsigned)k_split);
     k_gemm_q<TYPE, NB><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(a);
+    return (int)cudaGetLastError();
+}
+
+// uint8 planes of n_mat matrices [rows][row_bytes], mat_stride bytes apart (256-aligned): box = box_bytes x box_rows x 1 matrix
+int make_tmap_u8_3d(CUtensorMap * tm, const void * ptr, int64_t rows, int64_t row_bytes, int64_t n_mat, int64_t mat_stride, int box_bytes, int box_rows, bool swizzle128) {
+    encode_tiled_fn enc = get_encode(); if (!enc) return -1;
+    cuuint64_t dims[3] = {(cuuint64_t)row_bytes, (cuuint64_t)rows, (cuuint64_t)n_mat};
+    cuuint64_t strides[2] = {(cuuint64_t)row_bytes, (cuuint64_t)mat_stride};
+    cuuint32_t box[3] = {(cuuint32_t)box_bytes, (cuuint32_t)box_rows, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? 0 : -2;
+}
+
+// MoE: the segments' expert tensors (one 3-D map per plane covers every expert), row tiles of all segments on blockIdx.x, the tile table on blockIdx.y
+template <int TYPE, int NB>
+int launch_gemm_q_grouped(const b200q_moe_gemm & g, cudaStream_t st) {
+    using cfg = gemmq_cfg<TYPE, NB>;
+    gemmq_args a; memset(&a, 0, sizeof a);
+    b200q_layout L; if (b200q_make_layout(TYPE, g.M, g.K, &L)) return -1;
+    const int64_t p1_row = (g.K / 256) * cfg::P1, p2_row = (g.K / 256) * cfg::P2;
+    const int mt = (int)((g.M + BM - 1) / BM);
+    for (int i = 0; i < g.n_seg; ++i) {
+        const char * W = (const char *)g.W[i];
+        if (make_tmap_u8_3d(&a.tmP0[i], W + L.plane_off[0], g.M, g.K / 2, g.n_expert, L.total_bytes, 128, BM, true)) return -10;
+        if (make_tmap_u8_3d(&a.tmP1[i], W + L.plane_off[1], g.M, p1_row, g.n_expert, L.total_bytes, cfg::P1, BM, false)) return -13;
+        if (cfg::P2 && make_tmap_u8_3d(&a.tmP2[i], W + L.plane_off[2], g.M, p2_row, g.n_expert, L.total_bytes, cfg::P2, BM, false)) return -13;
+        a.seg[i].dst = g.dst[i]; a.seg[i].M = (int)g.M; a.seg[i].tile0 = i * mt;
+    }
+    if (make_tmap_bf16(&a.tmB, g.xb, g.n_rows, g.K, cfg::BN)) return -11;
+    a.n_seg = g.n_seg; a.N = (int)g.n_rows; a.K = (int)g.K; a.k_split = 1; a.rt = g.rt;
+    static bool configured[B200Q_MAX_DEVICES] = {};
+    const int dev = b200q_current_device();
+    if (!configured[dev]) {
+        if (cudaFuncSetAttribute(k_gemm_q<TYPE, NB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg::SMEM) != cudaSuccess) return -12;
+        configured[dev] = true;
+    }
+    const int64_t tiles = (g.n_rows + cfg::BN - 1) / cfg::BN + std::min<int64_t>(g.n_expert, g.n_rows);
+    dim3 grid((unsigned)(mt * g.n_seg), (unsigned)tiles, 1);
+    k_gemm_q<TYPE, NB, true><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(a);
     return (int)cudaGetLastError();
 }
 
@@ -878,7 +992,7 @@ int b200q_launch_f32_to_bf16(const float * x, int64_t x_stride, void * out, int6
     const int64_t xs = x_stride ? x_stride : K;
     if (K % 8 == 0 && xs % 4 == 0 && !((uintptr_t)x & 15) && !((uintptr_t)out & 15)) {
         const int64_t total8 = N * (K / 8); int64_t nb = (total8 + 256 * 4 - 1) / (256 * 4); if (nb > 132 * 8) nb = 132 * 8; if (nb < 1) nb = 1;
-        k_f32_to_bf16<<<(unsigned)nb, 256, 0, st>>>(x, xs, (__nv_bfloat16 *)out, K, N);
+        k_f32_to_bf16<false><<<(unsigned)nb, 256, 0, st>>>(x, xs, (__nv_bfloat16 *)out, K, N);
     } else {
         const int64_t total4 = N * (K / 4); int64_t nb = (total4 + 255) / 256; if (nb > 132 * 32) nb = 132 * 32; if (nb < 1) nb = 1;
         k_f32_to_bf16_k4<<<(unsigned)nb, 256, 0, st>>>(x, xs, (__nv_bfloat16 *)out, K, N);
@@ -927,6 +1041,46 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         int rc = b200q_launch_dequant_bf16(d.W[i], L, wscratch, st); if (rc) return rc;
         rc = bn256 ? launch_gemm_bf16<256>(wscratch, d.xb, d.dst[i], M, N, K, k_split, st) : launch_gemm_bf16<128>(wscratch, d.xb, d.dst[i], M, N, K, k_split, st);
         if (rc) return rc;
+    }
+    return 0;
+}
+
+int b200q_gemm_fused_type(int type) { return gemmq_supported(type) ? 1 : 0; }
+
+// MoE gather: bf16 [N][K] whose row n is row row_map[n] of x (rows K floats apart); a negative entry gives a zero row
+int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, void * out, int64_t K, int64_t N, cudaStream_t st) {
+    if (K % 8 || ((uintptr_t)x & 15) || ((uintptr_t)out & 15)) return -2;
+    const int64_t total8 = N * (K / 8); int64_t nb = (total8 + 256 * 4 - 1) / (256 * 4); if (nb > 132 * 8) nb = 132 * 8; if (nb < 1) nb = 1;
+    k_f32_to_bf16<true><<<(unsigned)nb, 256, 0, st>>>(x, K, (__nv_bfloat16 *)out, K, N, row_map);
+    return (int)cudaGetLastError();
+}
+
+// MoE grouped GEMM over the expert-sorted rows g.xb.  Types of the fused kernel: ONE launch over the row tiles of the segments, the weights
+// decoded inside the kernel.  Every other type: the experts are walked in groups whose bf16 copies fit `wscratch` (a contiguous range of the
+// sorted rows each); per group and segment the experts that received rows are dequantised, then one grouped bf16 GEMM.
+int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t ws_bytes, cudaStream_t st) {
+    if (g.K % 256 || g.n_seg < 1 || g.n_seg > 2 || g.n_rows < 1 || (g.bn != 128 && g.bn != 256)) return -2;
+    const bool bn256 = g.bn == 256;
+    if (gemmq_supported(g.type)) {
+        switch (g.type) {
+#define GQ(T) case T: return bn256 ? launch_gemm_q_grouped<T, 1>(g, st) : launch_gemm_q_grouped<T, 0>(g, st);
+            GQ(B200Q_TYPE_IQ4_NL) GQ(B200Q_TYPE_Q4_0) GQ(B200Q_TYPE_Q4_K) GQ(B200Q_TYPE_IQ4_K)
+            GQ(B200Q_TYPE_Q4_1) GQ(B200Q_TYPE_Q5_0) GQ(B200Q_TYPE_Q5_1) GQ(B200Q_TYPE_Q5_K) GQ(B200Q_TYPE_IQ5_K)
+#undef GQ
+            default: return -1;
+        }
+    }
+    b200q_layout L; if (b200q_make_layout(g.type, g.M, g.K, &L)) return -1;
+    const int64_t ebytes = g.M * g.K * 2;
+    const int64_t per = std::min<int64_t>(g.n_expert, (int64_t)(ws_bytes / (size_t)ebytes));
+    if (per < 1) return -5;
+    for (int e0 = 0; e0 < g.n_expert; e0 += (int)per) {
+        b200q_moe_route rt = g.rt; rt.e0 = e0; rt.e1 = (int)std::min<int64_t>(g.n_expert, e0 + per);
+        for (int i = 0; i < g.n_seg; ++i) {
+            int rc = b200q_launch_dequant_bf16_experts(g.W[i], L, wscratch, rt.e0, rt.e1 - rt.e0, g.rt.bounds, st); if (rc) return rc;
+            rc = bn256 ? launch_gemm_bf16_grouped<256>(wscratch, rt.e1 - rt.e0, g, g.dst[i], rt, st) : launch_gemm_bf16_grouped<128>(wscratch, rt.e1 - rt.e0, g, g.dst[i], rt, st);
+            if (rc) return rc;
+        }
     }
     return 0;
 }

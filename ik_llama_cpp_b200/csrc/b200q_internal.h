@@ -100,3 +100,24 @@ size_t b200q_gemm_i8_workspace_bytes(int64_t K, int64_t N);
 int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t x_stride, void * ws, size_t ws_bytes, cudaStream_t st);
 int b200q_launch_add_rows(const float * a, const float * b, float * dst, int64_t m, int64_t n, int64_t nb, cudaStream_t st);
 int b200q_launch_f32_to_bf16(const float * x, int64_t x_stride, void * out, int64_t K, int64_t N, cudaStream_t st);
+int b200q_gemm_fused_type(int type);
+
+// MoE prefill (b200q_moe.cu): routing tables of the expert-sorted slots, built on the device by k_moe_route and read by the grouped GEMMs.
+//   bounds[e] .. bounds[e+1]: the sorted rows of expert e;  slot[r]: the (token, slot) index t * n_used + u of sorted row r;
+//   tiles[tile_start[e] .. tile_start[e+1]): {e, first sorted row} of expert e's tiles of BN rows;  e0 .. e1: the experts a launch covers.
+struct b200q_moe_route { const int * bounds; const int * tile_start; const int2 * tiles; const int * slot; int e0, e1; };
+struct b200q_moe_gemm {
+    int type; int n_seg; const void * W[2]; float * dst[2];   // n_expert matrices [M x K] per segment, b200q_plane_bytes apart; dst f32 [slot][M]
+    int64_t M, K; int n_expert; int64_t n_rows;               // n_rows: rows of xb = number of slots (the routed rows are a prefix)
+    const void * xb; int bn;                                   // bf16 [n_rows][K] in expert-sorted order; tile width (128 / 256)
+    b200q_moe_route rt;
+};
+int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, void * out, int64_t K, int64_t N, cudaStream_t st);
+int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t ws_bytes, cudaStream_t st);
+// dequantise experts e0 .. e0+n_e-1 of an expert tensor (L: one expert; experts L.total_bytes apart) into bf16 [n_e][M][K]; with bounds, the experts
+// that received no rows are skipped
+int b200q_launch_dequant_bf16_experts(const void * W, const b200q_layout & L, void * out, int e0, int n_e, const int * bounds, cudaStream_t st);
+int b200q_launch_wire_dequant_bf16_experts(int type, const void * W, int64_t M, int64_t K, int64_t estride, void * out, int e0, int n_e, const int * bounds, cudaStream_t st);
+int b200q_moe_gemm_shape_ok(int type, int64_t M, int64_t K, int n_used, int nb1, int n_tokens, int n_expert, int up_gate);
+size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate);
+int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_bytes, cudaStream_t st);

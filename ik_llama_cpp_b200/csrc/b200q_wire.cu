@@ -18,8 +18,13 @@ int b200q_wire_check(int type, int64_t M, int64_t K);
 
 namespace {
 
+// blockIdx.y = expert e0 + y of an expert tensor (experts estride bytes apart) -> out[y][M][K], skipped when `bounds` says it received no rows
 template <int TYPE>
-__global__ void k_wire_dequant_bf16(const uint8_t * __restrict__ W, int64_t M, int64_t K, __nv_bfloat16 * __restrict__ out) {
+__global__ void k_wire_dequant_bf16(const uint8_t * __restrict__ W, int64_t M, int64_t K, __nv_bfloat16 * __restrict__ out,
+                                    int64_t estride, int e0, const int * __restrict__ bounds) {
+    const int e = e0 + (int)blockIdx.y;
+    if (bounds != nullptr && __ldg(bounds + e + 1) == __ldg(bounds + e)) return;
+    W += (int64_t)e * estride; out += (int64_t)blockIdx.y * M * K;
     const int64_t n32 = K / 32, total = M * n32;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t row = i / n32, it = i % n32;
@@ -213,11 +218,16 @@ int b200q_wire_check(int type, int64_t M, int64_t K) {
 }
 
 int b200q_launch_wire_dequant_bf16(int type, const void * W, int64_t M, int64_t K, void * out, cudaStream_t st) {
+    return b200q_launch_wire_dequant_bf16_experts(type, W, M, K, 0, out, 0, 1, nullptr, st);
+}
+int b200q_launch_wire_dequant_bf16_experts(int type, const void * W, int64_t M, int64_t K, int64_t estride, void * out, int e0, int n_e, const int * bounds, cudaStream_t st) {
     const int rc = b200q_wire_check(type, M, K); if (rc) return rc;
+    if (n_e < 1 || n_e > 65535) return -2;
     const int64_t total = M * (K / 32);
-    const int bs = 128; int64_t nb = (total + bs - 1) / bs; if (nb > 132 * 64) nb = 132 * 64; if (nb < 1) nb = 1;
+    const int bs = 128; int64_t nb = (total + bs - 1) / bs; const int64_t cap = 132 * 64 / n_e > 1 ? 132 * 64 / n_e : 1; if (nb > cap) nb = cap; if (nb < 1) nb = 1;
+    const dim3 grid((unsigned)nb, (unsigned)n_e);
     switch (type) {
-#define X(T) case T: k_wire_dequant_bf16<T><<<(unsigned)nb, bs, 0, st>>>((const uint8_t *)W, M, K, (__nv_bfloat16 *)out); break;
+#define X(T) case T: k_wire_dequant_bf16<T><<<grid, bs, 0, st>>>((const uint8_t *)W, M, K, (__nv_bfloat16 *)out, estride, e0, bounds); break;
         B200Q_FOR_WIRE_TYPES(X)
 #undef X
         default: return -1;

@@ -309,7 +309,7 @@ def mul_mat_id_workspace(w: ExpertTensor, n_tokens: int, n_used: int, nb1: int, 
 def mul_mat_id_gemm(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "ExpertTensor | None" = None, unary: str = "silu", limit: float = 0.0,
                     out: torch.Tensor | None = None) -> torch.Tensor:
     """GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE on the grouped tensor-core GEMM over expert-sorted slots (prefill), whatever the batch.
-    Same operands and result as mul_mat_id, except that ids outside [0, n_expert) give zero rows.  Routing stays on the device."""
+    Same operands and result as mul_mat_id (ids outside [0, n_expert) give zero rows on both).  Routing stays on the device."""
     _require_cuda()
     n_tokens, nb1, n_used = _mul_mat_id_args(w, x, ids, gate)
     dst = out if out is not None else torch.empty((n_tokens, n_used, w.m), dtype=torch.float32, device=x.device)

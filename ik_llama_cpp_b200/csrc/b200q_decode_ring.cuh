@@ -208,7 +208,11 @@ __global__ void __launch_bounds__(512, 1) k_mmvq_id(const mmvq_id_args a) {
     const int64_t total = (int64_t)a.n_slots * a.M;
     for (int64_t g = (int64_t)blockIdx.x * nwarps + warp; g < total; g += (int64_t)gridDim.x * nwarps) {
         const int s = (int)(g / a.M); const int64_t row = g - (int64_t)s * a.M;
-        int e = __ldg(a.ids + s); e = e < 0 ? 0 : (e >= a.n_expert ? a.n_expert - 1 : e);          // (a corrupt id must not read outside the tensor)
+        const int e = __ldg(a.ids + s);
+        if (e < 0 || e >= a.n_expert) {             // skipped slot (the -1 of ggml_top_k_thresh): a zero row, no weights read; s is warp-uniform
+            if (lane == 0) a.dst[(int64_t)s * a.M + row] = 0.0f;
+            continue;
+        }
         const int col = (s / a.n_used) * a.nb1 + (s % a.n_used) % a.nb1;
         b200q_planes P = a.P, P2 = a.P2;
 #pragma unroll

@@ -149,7 +149,11 @@ __global__ void __launch_bounds__(256) k_wire_mmvq_id(const wire_id_args a) {
     const int64_t total = (int64_t)a.n_slots * a.M;
     for (int64_t g = (int64_t)blockIdx.x * nwarps + warp; g < total; g += (int64_t)gridDim.x * nwarps) {
         const int s = (int)(g / a.M); const int64_t row = g - (int64_t)s * a.M;
-        int e = __ldg(a.ids + s); e = e < 0 ? 0 : (e >= a.n_expert ? a.n_expert - 1 : e);
+        const int e = __ldg(a.ids + s);
+        if (e < 0 || e >= a.n_expert) {             // skipped slot: a zero row, no weights read (s is warp-uniform)
+            if (lane == 0) a.dst[(int64_t)s * a.M + row] = 0.0f;
+            continue;
+        }
         const int col = (s / a.n_used) * a.nb1 + (s % a.n_used) % a.nb1;
         const int8_t * xq = sq + (size_t)col * K; const float * xd = sd + col * n32;
         float acc = 0.0f, acc2 = 0.0f;

@@ -159,14 +159,14 @@ B200Q_API int b200q_add_rows(const float * a, const float * b, float * dst, int6
  * ggml-cuda.cu:2836-3540; mul_mat_vec_q with ids, mmvq-templates.cuh:293-302).  W: n_expert matrices [m x k] of `type`, each in the device layout,
  * b200q_plane_bytes(type, m, k) apart; ids: DEVICE int32 [n_tokens][n_used]; x f32 [n_tokens][nb1][k] (nb1 = 1: the column is shared by the slots of
  * a token, nb1 = n_used: one column per slot); dst f32 [n_tokens][n_used][m]:  dst[t][e] = W[ids[t][e]] . x[t][e % nb1]
- * (W_gate != NULL: unary(W_gate[id] . x) * (W[id] . x)).  Expert ids are resolved on the device.  The quantised activation columns of a launch live
+ * (W_gate != NULL: unary(W_gate[id] . x) * (W[id] . x)); ids outside [0, n_expert) give zero rows, as in the reference.  Expert ids are resolved on the device.  The quantised activation columns of a launch live
  * in shared memory (200 KB of q8_1): batches whose n_tokens * nb1 columns exceed that are walked in token chunks by the same kernel. */
 B200Q_API int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
                          int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream);
 /* ---- MoE prefill: grouped wgmma GEMM over expert-sorted slots (the reference's mmq_id path, ggml-cuda.cu:2906-2910, 3210-3267) ----
  * Same arguments and result as b200q_mul_mat_id_vec, plus a device workspace.  Routing (counts, sort by expert, tile table) runs on the device: no
  * host round trip, no allocation, no synchronisation, so the call can be captured in a CUDA graph.  Ids outside [0, n_expert) are skipped and their
- * dst rows are ZERO (the reference's semantics; b200q_mul_mat_id_vec clamps them instead).  bf16 operands, f32 accumulation (as the dense GEMM).
+ * dst rows are ZERO (the reference's semantics, as in b200q_mul_mat_id_vec).  bf16 operands, f32 accumulation (as the dense GEMM).
  * b200q_mul_mat_id_workspace: bytes the grouped path needs, or 0 exactly when b200q_mul_mat_id takes the mat-vec path: an ineligible shape, or a
  * batch below the measured crossover (n_slots = n_tokens * n_used; up/gate: n_slots <= 5 * n_expert, else n_slots <= 32).  Needs no device.
  * b200q_mul_mat_id_gemm: always the grouped path (K % 256 == 0, n_expert <= 1024).  b200q_mul_mat_id: the dispatcher (workspace may be NULL when the

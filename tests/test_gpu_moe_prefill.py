@@ -28,9 +28,23 @@ def be():
     return backend
 
 
-def silu_glu(g, u):
-    g = np.asarray(g, np.float64)
-    return g / (1 + np.exp(-g)) * np.asarray(u, np.float64)
+def glu_ref(unary, g, u, limit=0.0):
+    """act(gate) * up with the reference's order of operations (the copy in test_gpu_parity.py): the clamp follows silu and exists for silu only;
+    swiglu_oai: alpha 1.702, limit 7."""
+    g = np.asarray(g, np.float64); u = np.asarray(u, np.float64)
+    if unary == "silu":
+        a = g / (1 + np.exp(-g))
+        if limit > 1e-6:
+            a = np.minimum(a, limit); u = np.clip(u, -limit, limit)
+        return a * u
+    if unary == "gelu":
+        return 0.5 * g * (1 + np.tanh(0.79788456080286535588 * g * (1 + 0.044715 * g * g))) * u
+    if unary == "relu":
+        return np.maximum(g, 0) * u
+    if unary == "swiglu_oai":
+        g = np.minimum(g, 7.0); u = np.clip(u, -7.0, 7.0)
+        return g / (1 + np.exp(-1.702 * g)) * (1 + u)
+    raise ValueError(unary)
 
 
 def experts(be, oracle, name, n_expert, m, k, seed):
@@ -39,7 +53,7 @@ def experts(be, oracle, name, n_expert, m, k, seed):
     return wires, be.set_expert_tensor(t, np.concatenate(wires), n_expert, m, k)
 
 
-def exact(oracle, name, wires, gwires, x, ids, m):
+def exact(oracle, name, wires, gwires, x, ids, m, unary="silu", limit=0.0):
     """dst[t, u] = W[ids[t, u]] . x[t, u % nb1] on the wire bytes (zero rows for ids out of range); one oracle call per expert"""
     t = GGML_TYPE[name]
     n_tokens, nb1, _ = x.shape
@@ -53,7 +67,7 @@ def exact(oracle, name, wires, gwires, x, ids, m):
         xe = cols[tk * nb1 + u % nb1]
         r = oracle.mul_mat_exact(t, wires[e], xe, m).astype(np.float64)
         if gwires is not None:
-            r = silu_glu(oracle.mul_mat_exact(t, gwires[e], xe, m), r)
+            r = glu_ref(unary, oracle.mul_mat_exact(t, gwires[e], xe, m), r, limit)
         y[tk, u] = r
     return y
 
@@ -62,17 +76,30 @@ def exact(oracle, name, wires, gwires, x, ids, m):
 @pytest.mark.parametrize("nb1", [1, 2])
 @pytest.mark.parametrize("glu", [False, True])
 def test_grouped_gemm_vs_oracle(be, oracle, name, nb1, glu):
+    check_grouped_gemm(be, oracle, name, nb1, glu, "silu", 0.0)
+
+
+@pytest.mark.parametrize("name", FUSED_TYPES + GENERIC_TYPES)
+@pytest.mark.parametrize("nb1", [1, 2])
+@pytest.mark.parametrize("unary,limit", [("silu", 1.5), ("gelu", 0.0), ("relu", 0.0), ("swiglu_oai", 0.0)])
+def test_grouped_gemm_glu_unary(be, oracle, name, nb1, unary, limit):
+    """MOE_FUSED_UP_GATE on the grouped GEMM with the other GLUs of the reference (plain silu: test_grouped_gemm_vs_oracle).  limit (silu only)
+    clamps most outputs of these shapes, so its NMSE bar follows test_gpu_parity.py::test_fused_up_gate_gemm: 1e-3."""
+    check_grouped_gemm(be, oracle, name, nb1, True, unary, limit)
+
+
+def check_grouped_gemm(be, oracle, name, nb1, glu, unary, limit):
     n_expert, n_used, m, k, n_tokens = 8, 2, 260, 1024, 96           # M = 260: a partial 128-row tile per expert
     wires, W = experts(be, oracle, name, n_expert, m, k, 700)
     gwires, G = experts(be, oracle, name, n_expert, m, k, 800) if glu else (None, None)
     rng = np.random.default_rng(11 + nb1)
     x = rng.standard_normal((n_tokens, nb1, k)).astype(np.float32)
     ids = np.stack([rng.permutation(n_expert)[:n_used] for _ in range(n_tokens)]).astype(np.int32)
-    y = be.mul_mat_id_gemm(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G).cpu().numpy()
-    e = nmse(y, exact(oracle, name, wires, gwires, x, ids, m))
-    assert e <= (2e-4 if glu else 2e-5), f"{name} nb1={nb1} glu={glu}: NMSE {e}"
+    y = be.mul_mat_id_gemm(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G, unary=unary, limit=limit).cpu().numpy()
+    e = nmse(y, exact(oracle, name, wires, gwires, x, ids, m, unary, limit))
+    assert e <= (2e-5 if not glu else 2e-4 if limit == 0 else 1e-3), f"{name} nb1={nb1} glu={glu} {unary} {limit}: NMSE {e}"
     # the dispatcher takes the grouped path for this batch (96 * 2 slots > 8 per expert) and gives the same bits
-    yd = be.mul_mat_id_dispatch(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G).cpu().numpy()
+    yd = be.mul_mat_id_dispatch(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G, unary=unary, limit=limit).cpu().numpy()
     assert np.array_equal(y, yd)
 
 
@@ -133,6 +160,42 @@ def test_skipped_ids_give_zero_rows_with_glu(be, oracle):
     assert np.all(y[::7, 1] == 0.0)
     ok = ids >= 0
     assert nmse(y[ok], exact(oracle, "Q4_K", wires, gwires, x, ids, m)[ok]) <= 2e-4
+
+
+@pytest.mark.parametrize("name", ["IQ4_NL", "IQ2_XXS"])
+@pytest.mark.parametrize("glu", [False, True])
+def test_skipped_ids_give_zero_rows_on_both_sides_of_the_dispatch_threshold(be, oracle, name, glu):
+    """One set of ids with -1 and n_expert in some slots, at the last batch the dispatcher gives the mat-vec kernel (k_mmvq_id / k_wire_mmvq_id) and
+    the first one it gives the grouped GEMM (thresholds mirrored by test_moe_dispatch.py): zero rows on both sides, the valid rows within each path's
+    bar (mat-vec: 5e-5 of the rms against the q8_1 oracle, as test_gpu_parity.py::test_mul_mat_id; grouped: NMSE against the exact product)."""
+    from test_moe_dispatch import last_mat_vec_batch
+    t = GGML_TYPE[name]
+    n_expert, n_used, m, k = 8, 2, 256, 512
+    t_last = last_mat_vec_batch(n_expert, n_used, glu)
+    wires, W = experts(be, oracle, name, n_expert, m, k, 1700)
+    gwires, G = experts(be, oracle, name, n_expert, m, k, 1800) if glu else (None, None)
+    rng = np.random.default_rng(17)
+    x = rng.standard_normal((t_last + 1, 1, k)).astype(np.float32)
+    ids = np.stack([rng.permutation(n_expert)[:n_used] for _ in range(t_last + 1)]).astype(np.int32)
+    ids[0, 1] = -1
+    ids[3, 0] = n_expert
+    ids[t_last - 1, 1] = -1
+    for n_tokens, grouped in ((t_last, False), (t_last + 1, True)):
+        assert (be.mul_mat_id_workspace(W, n_tokens, n_used, 1, glu) > 0) == grouped
+        xs, ids_n = x[:n_tokens], ids[:n_tokens]
+        y = be.mul_mat_id_dispatch(W, torch.from_numpy(xs).cuda(), torch.from_numpy(ids_n).cuda(), gate=G).cpu().numpy()
+        invalid = (ids_n < 0) | (ids_n >= n_expert)
+        assert np.all(y[invalid] == 0.0), f"n_tokens={n_tokens}: skipped slots must give zero rows"
+        if grouped:
+            e = nmse(y[~invalid], exact(oracle, name, wires, gwires, xs, ids_n, m)[~invalid])
+            assert e <= (2e-4 if glu else 2e-5), f"grouped side: NMSE {e}"
+            continue
+        for tk, u in zip(*np.nonzero(~invalid)):
+            col = xs[tk, 0][None, :]
+            ref = oracle.mul_mat_q8_1(t, wires[ids_n[tk, u]], col, m, variant="b200")[0].astype(np.float64)
+            if glu:
+                ref = glu_ref("silu", oracle.mul_mat_q8_1(t, gwires[ids_n[tk, u]], col, m, variant="b200")[0].astype(np.float64), ref)
+            assert np.abs(y[tk, u] - ref).max() <= 5e-5 * np.sqrt((ref ** 2).mean()), (tk, u)
 
 
 @pytest.mark.parametrize("name", ["IQ4_NL", "IQ2_XXS"])

@@ -268,12 +268,29 @@ def test_mat_vec_bias(be, oracle, name, n):
     assert np.abs(y.cpu().numpy() - yq).max() <= 2e-5 * rms(yq)
 
 
-@pytest.mark.parametrize("name", ["IQ4_NL", "Q4_K", "Q6_K", "IQ2_K", "IQ4_KS", "IQ2_XXS", "IQ3_S", "IQ4_K_R4", "IQ2_KT"])
-@pytest.mark.parametrize("n_tokens,nb1", [(1, 1), (1, 3), (4, 1), (3, 3)])
+MUL_MAT_ID_TYPES = ["IQ4_NL", "Q4_K", "Q6_K", "IQ2_K", "IQ4_KS", "IQ2_XXS", "IQ3_S", "IQ4_K_R4", "IQ2_KT"]
+MUL_MAT_ID_SHAPES = [(1, 1), (1, 3), (4, 1), (3, 3)]
+
+
+@pytest.mark.parametrize("name", MUL_MAT_ID_TYPES)
+@pytest.mark.parametrize("n_tokens,nb1", MUL_MAT_ID_SHAPES)
 @pytest.mark.parametrize("glu", [False, True])
 def test_mul_mat_id(be, oracle, name, n_tokens, nb1, glu):
     """GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE for decode-sized batches: expert ids are resolved on the device, one launch.
-    Oracle: the plain mat-vec oracle on the selected expert's wire bytes."""
+    Oracle: the plain mat-vec oracle on the selected expert's wire bytes.  Ids -1 (ggml_top_k_thresh) and n_expert are skipped: exact zero rows,
+    as in the reference and on the grouped prefill path."""
+    check_mul_mat_id(be, oracle, name, n_tokens, nb1, glu, "silu", 0.0)
+
+
+@pytest.mark.parametrize("name", MUL_MAT_ID_TYPES)
+@pytest.mark.parametrize("n_tokens,nb1", MUL_MAT_ID_SHAPES)
+@pytest.mark.parametrize("unary,limit", [("silu", 1.5), ("gelu", 0.0), ("relu", 0.0), ("swiglu_oai", 0.0)])
+def test_mul_mat_id_glu_unary(be, oracle, name, n_tokens, nb1, unary, limit):
+    """MOE_FUSED_UP_GATE on the mat-vec kernel with the other GLUs of the reference (plain silu: test_mul_mat_id), skipped ids included."""
+    check_mul_mat_id(be, oracle, name, n_tokens, nb1, True, unary, limit)
+
+
+def check_mul_mat_id(be, oracle, name, n_tokens, nb1, glu, unary, limit):
     t = GGML_TYPE[name]
     n_expert, n_used, m, k = 6, 3, 260, 1024
     rs = len(make_wire(oracle, name, 4, k, seed=1)) // 4
@@ -285,14 +302,19 @@ def test_mul_mat_id(be, oracle, name, n_tokens, nb1, glu):
     rng = np.random.default_rng(77 + n_tokens + nb1)
     x = rng.standard_normal((n_tokens, nb1, k)).astype(np.float32)
     ids = np.stack([rng.permutation(n_expert)[:n_used] for _ in range(n_tokens)]).astype(np.int32)
-    y = be.mul_mat_id(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G, unary="silu").cpu().numpy()
+    ids[0, 1] = -1
+    ids[-1, 2] = n_expert
+    y = be.mul_mat_id(W, torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda(), gate=G, unary=unary, limit=limit).cpu().numpy()
     assert y.shape == (n_tokens, n_used, m)
     for tk in range(n_tokens):
         for e in range(n_used):
+            if not 0 <= ids[tk, e] < n_expert:
+                assert np.all(y[tk, e] == 0.0), (tk, e, ids[tk, e])
+                continue
             col = x[tk, e % nb1][None, :]
             ref = oracle.mul_mat_q8_1(t, wires[ids[tk, e]], col, m, variant="b200")[0].astype(np.float64)
             if glu:
-                ref = glu_ref("silu", oracle.mul_mat_q8_1(t, gwires[ids[tk, e]], col, m, variant="b200")[0].astype(np.float64), ref)
+                ref = glu_ref(unary, oracle.mul_mat_q8_1(t, gwires[ids[tk, e]], col, m, variant="b200")[0].astype(np.float64), ref, limit)
             assert np.abs(y[tk, e] - ref).max() <= 5e-5 * max(rms(ref), 1e-30), (tk, e)
 
 
@@ -339,11 +361,12 @@ def test_gemm_vs_oracle(be, oracle, ref_or_none, name, n):
         assert e <= 2e-5, f"{name} n={n}: NMSE {e}"      # ours: bf16 inputs, f32 accumulate
 
 
-@pytest.mark.parametrize("m,k,n", [(384, 1024, 512), (130, 3200, 40), (256, 8640, 70), (128, 64, 16)])
+@pytest.mark.parametrize("m,k,n", [(384, 1024, 512), (384, 1024, 300), (130, 3200, 40), (256, 8640, 70), (128, 64, 16)])
 def test_bitnet_int8_gemm_is_exact_integer_arithmetic(be, oracle, m, k, n):
     """IQ2_BN prefill = wgmma u8 x s8 on per-token int8 activations: dst = rs[m] * ts[n] * (sum_k q*xq - sum_k xq) with exact integer sums.
     Emulated in numpy (same quantiser: ts = amax/127, xq = rint(x / ts)): only the two f32 multiplies of the epilogue may round.  K = 3200 / 8640 are the
-    bitnet-b1.58 row lengths (not multiples of the 128-wide k-block: zero-filled TMA tails), K = 64 a single wire block."""
+    bitnet-b1.58 row lengths (not multiples of the 128-wide k-block: zero-filled TMA tails), K = 64 a single wire block; N = 300 runs the BN = 256
+    instantiation with a ragged last column tile (44 of 256 columns)."""
     import ik_llama_cpp_b200 as pkg
     t = GGML_TYPE["IQ2_BN"]
     wire = make_wire(oracle, "IQ2_BN", m, k, seed=400 + n)

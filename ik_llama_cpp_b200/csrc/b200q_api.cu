@@ -63,7 +63,6 @@ constexpr size_t STAGE_KEEP = (size_t)64 << 20;      // upload staging above thi
 thread_local scratch g_x, g_y, g_ws, g_stage;
 // programmatic dependent launch for the decode kernels (default on; B200Q_PDL=0 or b200q_set_option("pdl",0) disables)
 int & opt_ring() { static int v = [] { const char * e = getenv("B200Q_RING"); return e ? atoi(e) : 1; }(); return v; }
-int & opt_fuse_epi() { static int v = [] { const char * e = getenv("B200Q_FUSE_EPILOGUE"); return e ? atoi(e) : 0; }(); return v; }
 int & opt_fused() { static int v = [] { const char * e = getenv("B200Q_FUSED_GEMM"); return e ? atoi(e) : 1; }(); return v; }
 // L2 warm-up of the next launch's weights: measured slower (the prefetch competes with the running kernel's own stream) -> opt-in
 int & opt_pf() { static int v = [] { const char * e = getenv("B200Q_PREFETCH_NEXT"); return e ? atoi(e) : 0; }(); return v; }
@@ -81,7 +80,6 @@ int b200q_set_option(const char * key, int value) {
     if (key && !strcmp(key, "q8_handoff")) { opt_q8() = value; return B200Q_OK; }
     if (key && !strcmp(key, "ring")) { opt_ring() = value; return B200Q_OK; }
     if (key && !strcmp(key, "fused_gemm")) { opt_fused() = value; return B200Q_OK; }
-    if (key && !strcmp(key, "fuse_epilogue")) { opt_fuse_epi() = value; return B200Q_OK; }
     return fail(B200Q_E_ARG, "b200q_set_option: unknown option");
 }
 int b200q_device_count(void) { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) return 0; return n; }
@@ -339,25 +337,10 @@ int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_ga
     if (workspace_bytes < up_bytes) return fail(B200Q_E_ARG, "b200q_fused_up_gate_gemm_bf16: workspace too small");
     float * up_res = (float *)workspace; void * wsc = (char *)workspace + up_bytes; const size_t wsc_bytes = workspace_bytes - up_bytes;
     cudaStream_t st = (cudaStream_t)stream;
-    int rc;
-    if (!b200q_gemm_epilogue_fusable(type, m, k, n, di.sm_count, opt_fused() && opt_fuse_epi() ? 2 : 0)) {
-        // default: up and gate as the two segments of ONE launch (up -> workspace, gate -> dst), then the unary-mul tail in place
-        b200q_gemm_multi d; memset(&d, 0, sizeof d);
-        d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n; d.xb = x_bf16;
-        rc = check_launch(b200q_launch_gemm_multi_bf16x(d, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(up,gate)");
-        if (rc) return rc;
-        return check_launch(b200q_launch_mul_unary(dst, up_res, dst, dst_bf16, m * n, unary, limit, st), "b200q_fused_up_gate_gemm_bf16(unary)");
-    }
-    rc = check_launch(b200q_launch_gemm_bf16x(type, W_up, x_bf16, up_res, m, k, n, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(up)");
-    if (rc) return rc;
-    if (b200q_gemm_epilogue_fusable(type, m, k, n, di.sm_count, opt_fused() && opt_fuse_epi() ? 2 : 0)) {
-        // gate GEMM whose epilogue applies unary(gate) * up and (optionally) emits the bf16 operand of ffn_down
-        b200q_gemm_multi d; memset(&d, 0, sizeof d);
-        d.type = type; d.n_seg = 1; d.W[0] = W_gate; d.dst[0] = dst; d.mul[0] = up_res; d.dst_bf[0] = dst_bf16; d.M[0] = m; d.K = k; d.N = n; d.xb = x_bf16;
-        d.act = unary; d.limit = limit;
-        return check_launch(b200q_launch_gemm_multi_bf16x(d, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(gate)");
-    }
-    rc = check_launch(b200q_launch_gemm_bf16x(type, W_gate, x_bf16, dst, m, k, n, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(gate)");
+    // up and gate as the two segments of ONE launch (up -> workspace, gate -> dst), then the unary-mul tail in place, which also writes dst_bf16
+    b200q_gemm_multi d; memset(&d, 0, sizeof d);
+    d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n; d.xb = x_bf16;
+    const int rc = check_launch(b200q_launch_gemm_multi_bf16x(d, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(up,gate)");
     if (rc) return rc;
     return check_launch(b200q_launch_mul_unary(dst, up_res, dst, dst_bf16, m * n, unary, limit, st), "b200q_fused_up_gate_gemm_bf16(unary)");
 }
@@ -368,10 +351,9 @@ int b200q_fused_up_gate(int type, const void * W_up, const void * W_gate, const 
     if ((m * n) % 4) return fail(B200Q_E_SHAPE, "b200q_fused_up_gate: m*n must be a multiple of 4");
     int rc;
     {   // ternary weights: both GEMMs on the int8 tensor pipe (one activation quantisation, one launch over the up and gate row tiles), then the unary-mul tail
-        static const int use_i8 = [] { const char * e = getenv("B200Q_BN_INT8"); return e ? atoi(e) : 1; }();
         dev_info & di = device_info();
         const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
-        if (type == B200Q_TYPE_IQ2_BN && use_i8 && opt_fused() && di.ok && workspace_bytes >= up_bytes + b200q_gemm_i8_workspace_bytes(k, n)) {
+        if (type == B200Q_TYPE_IQ2_BN && opt_fused() && di.ok && workspace_bytes >= up_bytes + b200q_gemm_i8_workspace_bytes(k, n)) {
             float * up_res = (float *)workspace;
             b200q_gemm_multi d; memset(&d, 0, sizeof d);
             d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n;

@@ -85,8 +85,8 @@ int b200q_launch_wire_dequant_bf16(int type, const void * W, int64_t M, int64_t 
 
 // prefill: up to 3 weight tensors of one type / K that share the bf16 activation operand xb [N][K]
 struct b200q_gemm_multi {
-    int type; int n_seg; const void * W[3]; float * dst[3]; const float * mul[3]; void * dst_bf[3]; int64_t M[3];
-    int64_t K, N; const void * xb; int act; float limit;
+    int type; int n_seg; const void * W[3]; float * dst[3]; int64_t M[3];
+    int64_t K, N; const void * xb;
 };
 size_t b200q_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t N);
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
@@ -95,7 +95,6 @@ int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * d
                             void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_mul_unary(const float * gate, const float * up, float * dst, void * dst_bf16, int64_t total, int act, float limit, cudaStream_t st);
-int b200q_gemm_epilogue_fusable(int type, int64_t M, int64_t K, int64_t N, int sm_count, int fused);
 size_t b200q_gemm_i8_workspace_bytes(int64_t K, int64_t N);
 int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t x_stride, void * ws, size_t ws_bytes, cudaStream_t st);
 int b200q_launch_add_rows(const float * a, const float * b, float * dst, int64_t m, int64_t n, int64_t nb, cudaStream_t st);

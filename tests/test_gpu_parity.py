@@ -382,7 +382,7 @@ def test_bitnet_int8_gemm_is_exact_integer_arithmetic(be, oracle, m, k, n):
     emul = (xq.astype(np.float64) * ts.astype(np.float64)) @ wd.T
     assert np.abs(y - emul).max() <= 4e-7 * np.abs(emul).max() + 1e-30, float(np.abs(y - emul).max() / np.abs(emul).max())
     assert nmse(y, oracle.mul_mat_exact(t, wire, x, m)) <= 3e-4
-    # the bf16 tensor-pipe path (B200Q_BN_INT8=0 equivalent: fused_gemm off) still agrees with exact math to bf16 accuracy
+    # the bf16 tensor-pipe path (fused_gemm off) still agrees with exact math to bf16 accuracy
     pkg.lib().b200q_set_option(b"fused_gemm", 0)
     try:
         y0 = be.mul_mat(w, torch.from_numpy(x).cuda()).cpu().numpy()
@@ -438,10 +438,9 @@ def test_gemm_multi_tensor_launch_qkv(be, oracle, name, n):
 
 @pytest.mark.parametrize("name,m,k", [("IQ4_NL", 1000, 256), ("IQ4_NL", 384, 1024), ("Q4_K", 1000, 256), ("Q6_K", 384, 1024), ("IQ2_BN", 256, 512)])
 @pytest.mark.parametrize("unary,limit", [("silu", 0.0), ("gelu", 0.0), ("relu", 0.0), ("silu", 1.5), ("swiglu_oai", 0.0)])
-@pytest.mark.parametrize("fuse", [0, 1])
-def test_fused_up_gate_gemm(be, oracle, name, m, k, unary, limit, fuse):
-    """GGML_OP_FUSED_UP_GATE for n > 8.  fuse=1 with k=256 (split-K 1): unary-mul inside the gate GEMM's epilogue; everything else:
-    gate GEMM + k_mul_unary.  Checked against act(gate.x)*(up.x) from the plain GEMM entry point and the oracle."""
+def test_fused_up_gate_gemm(be, oracle, name, m, k, unary, limit):
+    """GGML_OP_FUSED_UP_GATE for n > 8: up and gate in one GEMM launch + k_mul_unary.  Checked against act(gate.x)*(up.x) from the plain
+    GEMM entry point and the oracle."""
     t = GGML_TYPE[name]
     n = 70
     wu, wg = make_wire(oracle, name, m, k, seed=131), make_wire(oracle, name, m, k, seed=132)
@@ -450,13 +449,8 @@ def test_fused_up_gate_gemm(be, oracle, name, m, k, unary, limit, fuse):
     xg = torch.from_numpy(x).cuda()
     xb = be.convert_activations(xg)
     ybf = torch.empty((n, m), dtype=torch.bfloat16, device="cuda")
-    import ik_llama_cpp_b200 as pkg
-    pkg.lib().b200q_set_option(b"fuse_epilogue", fuse)       # 1: unary-mul inside the gate GEMM's epilogue (opt-in), 0: k_mul_unary tail
-    try:
-        y = be.fused_up_gate(up, gate, xg, unary=unary, limit=limit, x_bf16=xb, out_bf16=ybf)
-        y2 = be.fused_up_gate(up, gate, xg, unary=unary, limit=limit)           # f32 activations, no bf16 copy
-    finally:
-        pkg.lib().b200q_set_option(b"fuse_epilogue", 0)
+    y = be.fused_up_gate(up, gate, xg, unary=unary, limit=limit, x_bf16=xb, out_bf16=ybf)
+    y2 = be.fused_up_gate(up, gate, xg, unary=unary, limit=limit)           # f32 activations, no bf16 copy
     u, g = be.mul_mat(up, xg, x_bf16=xb).double(), be.mul_mat(gate, xg, x_bf16=xb).double()
     ref = torch.from_numpy(glu_ref(unary, g.cpu().numpy(), u.cpu().numpy(), limit)).cuda()
     scale = float(ref.pow(2).mean().sqrt())

@@ -25,7 +25,8 @@ at K = 53248, L = 26 (long rows) or 52 (LDG), u sqrt(L + 7) <= 4.6e-7, and the l
 seventh of the bar.  test_f32_kernel_order_stays_inside_the_bar replays both summation orders in f32 on the oracle's own terms at that K.
 The worst case without cancellation, gamma_{L+7} sum |v_i|, would exceed the bar at that K; it is not the case the data can produce.
 
-Skipped MoE slots, MoE mat-vecs and the tensor-parallel instantiations are covered elsewhere (test_gpu_parity.py, test_gpu_tp.py).
+The MoE mat-vecs (k_mmvq_id, k_wire_mmvq_id, skipped slots included) have their own table and sweep in test_gpu_moe_decode.py, which reuses the
+bars, the profiler and the child-process runner of this file; the tensor-parallel instantiations are covered in test_gpu_tp.py.
 """
 import json
 import os
@@ -286,7 +287,7 @@ for _name in ("IQ2_XXS", "IQ4_KT", "IQ1_S_R4"):
                       [wire(_name, 1, False, 272), wire(_name, 2, False, 272), wire(_name, 4, False, 272), wire(_name, 1, False, 272),
                        wire(_name, 8, False, 264), wire(_name, 1, True, 272)]))
 
-KERNEL_RE = re.compile(r"\b(k_mmvq_ring|k_mmvq|k_wire_mmvq|k_gemm_q|k_gemm_bf16)<([^<>]*)>")
+KERNEL_RE = re.compile(r"\b(k_mmvq_ring|k_mmvq_id|k_mmvq|k_wire_mmvq_id|k_wire_mmvq|k_gemm_q|k_gemm_bf16)<([^<>]*)>")
 
 
 def matmul_launches(kernels):
@@ -391,9 +392,10 @@ def _child(case_id, out_dir):
                    "sms": torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count}, f)
 
 
-def run_child(case_id, out_dir):
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), case_id, str(out_dir)], capture_output=True, text=True,
-                       env=dict(os.environ), cwd=ROOT, timeout=600)
+def run_child(case_id, out_dir, script=__file__, env=None):
+    """Run `script <case_id> <out_dir>` (a test module whose __main__ writes y.npz and launches.json there), with `env` added to the environment."""
+    r = subprocess.run([sys.executable, os.path.abspath(script), case_id, str(out_dir)], capture_output=True, text=True,
+                       env={**os.environ, **(env or {})}, cwd=ROOT, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
     with open(os.path.join(out_dir, "launches.json")) as f:
         got = json.load(f)

@@ -315,7 +315,8 @@ def check_mul_mat_id(be, oracle, name, n_tokens, nb1, glu, unary, limit):
             ref = oracle.mul_mat_q8_1(t, wires[ids[tk, e]], col, m, variant="b200")[0].astype(np.float64)
             if glu:
                 ref = glu_ref(unary, oracle.mul_mat_q8_1(t, gwires[ids[tk, e]], col, m, variant="b200")[0].astype(np.float64), ref, limit)
-            assert np.abs(y[tk, e] - ref).max() <= 5e-5 * max(rms(ref), 1e-30), (tk, e)
+            # plain: the dense mat-vec bar (same arithmetic per slot, test_gpu_moe_decode.py); GLU: the fused up/gate bar
+            assert np.abs(y[tk, e] - ref).max() <= (5e-5 if glu else 2e-5) * max(rms(ref), 1e-30), (tk, e)
 
 
 def test_mul_mat_id_token_chunks(be):

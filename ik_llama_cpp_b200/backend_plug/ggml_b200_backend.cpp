@@ -66,28 +66,48 @@ GGML_CALL static void b200_buffer_memset_tensor(ggml_backend_buffer_t buffer, gg
     b200_buffer_ctx * c = (b200_buffer_ctx *)buffer->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
     B200_CUDA_CHECK(cudaMemsetAsync((char *)t->data + off, v, size, cudaStreamPerThread)); B200_CUDA_CHECK(cudaStreamSynchronize(cudaStreamPerThread));
 }
+// A view of a repacked tensor (a row slice of a merged weight ...) addresses wire-byte offsets, but the bytes under it are in the plane layout: its
+// host transfers go through the parent's wire image (b200_wire_rows), never raw.
+static const ggml_tensor * b200_repacked_parent(const ggml_tensor * t) { return t->view_src && b200_tensor_is_repacked(t->view_src) ? t->view_src : nullptr; }
+static bool b200_wire_staged(const ggml_tensor * t) { return b200_tensor_is_repacked(t) || b200_repacked_parent(t); }
+// Wire bytes [lo, lo + size) of the repacked tensor p, in whole rows.  3-D tensors (MoE experts [K, M, E]): every [M x K] matrix is re-laid-out on its
+// own, matrices are b200q_plane_bytes(M, K) apart.  A whole matrix moves directly; a part of one is staged through its unrepacked wire image on the
+// host: get copies the range out of it, set overwrites the range and re-lays the matrix out.  Anything but whole rows aborts.
+static void b200_wire_rows(const ggml_tensor * p, size_t lo, size_t size, void * get_dst, const void * set_src) {
+    const size_t row = ggml_row_size(p->type, p->ne[0]);
+    if (lo % row != 0 || size % row != 0 || lo + size > ggml_nbytes(p)) {
+        b200_log(GGML_LOG_LEVEL_ERROR, "%s: bytes [%zu, %zu) of %s are not whole rows of %zu bytes: a part of a quantized weight is only accessible in whole rows\n",
+                 __func__, lo, lo + size, p->name, row);
+        GGML_ABORT("b200: partial access to a repacked tensor");
+    }
+    const int64_t m = p->ne[1], k = p->ne[0], nmat = p->ne[2] * p->ne[3];
+    const size_t wire_mat = ggml_nbytes(p) / (size_t)nmat, dev_mat = (size_t)b200q_plane_bytes(p->type, m, k);
+    std::vector<char> stage;
+    for (int64_t e = (int64_t)(lo / wire_mat); e < nmat && (size_t)e * wire_mat < lo + size; ++e) {
+        const size_t a = lo > e * wire_mat ? lo : e * wire_mat, b = lo + size < (e + 1) * wire_mat ? lo + size : (e + 1) * wire_mat;
+        char * dev = (char *)p->data + e * dev_mat; char * host = (char *)(get_dst ? get_dst : (void *)set_src) + (a - lo);
+        if (b - a == wire_mat) {        // original GGUF bytes, bit-for-bit
+            B200Q_CHECK(get_dst ? b200q_get_tensor(p->type, dev, host, m, k, cudaStreamPerThread) : b200q_set_tensor(p->type, host, dev, m, k, cudaStreamPerThread));
+            continue;
+        }
+        stage.resize(wire_mat);
+        B200Q_CHECK(b200q_get_tensor(p->type, dev, stage.data(), m, k, cudaStreamPerThread));
+        if (get_dst) { memcpy(host, stage.data() + (a - e * wire_mat), b - a); continue; }
+        memcpy(stage.data() + (a - e * wire_mat), host, b - a);
+        B200Q_CHECK(b200q_set_tensor(p->type, stage.data(), dev, m, k, cudaStreamPerThread));
+    }
+}
 GGML_CALL static void b200_buffer_set_tensor(ggml_backend_buffer_t buffer, ggml_tensor * t, const void * data, size_t off, size_t size) {
     b200_buffer_ctx * c = (b200_buffer_ctx *)buffer->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
-    if (b200_tensor_is_repacked(t)) {
-        GGML_ASSERT(off == 0 && size == ggml_nbytes(t) && "quantized tensors are uploaded whole (they are re-laid-out on the device)");
-        // 3-D tensors (MoE experts [K, M, E]): every [M x K] matrix is re-laid-out on its own, matrices are b200q_plane_bytes(M, K) apart
-        const int64_t nmat = t->ne[2] * t->ne[3]; const size_t wire_mat = ggml_nbytes(t) / (size_t)nmat, dev_mat = (size_t)b200q_plane_bytes(t->type, t->ne[1], t->ne[0]);
-        for (int64_t e = 0; e < nmat; ++e)
-            B200Q_CHECK(b200q_set_tensor(t->type, (const char *)data + e * wire_mat, (char *)t->data + e * dev_mat, t->ne[1], t->ne[0], cudaStreamPerThread));
-        return;
-    }
+    if (b200_tensor_is_repacked(t)) { b200_wire_rows(t, off, size, nullptr, data); return; }
+    if (const ggml_tensor * p = b200_repacked_parent(t)) { b200_wire_rows(p, t->view_offs + off, size, nullptr, data); return; }
     B200_CUDA_CHECK(cudaMemcpyAsync((char *)t->data + off, data, size, cudaMemcpyHostToDevice, cudaStreamPerThread));
     B200_CUDA_CHECK(cudaStreamSynchronize(cudaStreamPerThread));
 }
 GGML_CALL static void b200_buffer_get_tensor(ggml_backend_buffer_t buffer, const ggml_tensor * t, void * data, size_t off, size_t size) {
     b200_buffer_ctx * c = (b200_buffer_ctx *)buffer->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
-    if (b200_tensor_is_repacked(t)) {
-        GGML_ASSERT(off == 0 && size == ggml_nbytes(t));
-        const int64_t nmat = t->ne[2] * t->ne[3]; const size_t wire_mat = ggml_nbytes(t) / (size_t)nmat, dev_mat = (size_t)b200q_plane_bytes(t->type, t->ne[1], t->ne[0]);
-        for (int64_t e = 0; e < nmat; ++e)      // original GGUF bytes, bit-for-bit
-            B200Q_CHECK(b200q_get_tensor(t->type, (const char *)t->data + e * dev_mat, (char *)data + e * wire_mat, t->ne[1], t->ne[0], cudaStreamPerThread));
-        return;
-    }
+    if (b200_tensor_is_repacked(t)) { b200_wire_rows(t, off, size, data, nullptr); return; }
+    if (const ggml_tensor * p = b200_repacked_parent(t)) { b200_wire_rows(p, t->view_offs + off, size, data, nullptr); return; }
     B200_CUDA_CHECK(cudaMemcpyAsync(data, (const char *)t->data + off, size, cudaMemcpyDeviceToHost, cudaStreamPerThread));
     B200_CUDA_CHECK(cudaStreamSynchronize(cudaStreamPerThread));
 }
@@ -98,6 +118,7 @@ static size_t b200_alloc_size(const ggml_tensor * t) {
 }
 GGML_CALL static bool b200_buffer_cpy_tensor(ggml_backend_buffer_t buffer, const ggml_tensor * src, ggml_tensor * dst) {
     if (!src->buffer || !b200_buffer_is_ours(src->buffer)) return false;       // host sources go through set_tensor
+    if (b200_repacked_parent(src) || b200_repacked_parent(dst)) return false;  // views of repacked tensors go through the wire image
     if (src->type != dst->type || ggml_nbytes(src) != ggml_nbytes(dst) || b200_alloc_size(src) != b200_alloc_size(dst)) return false;    // same layout on both sides only
     b200_buffer_ctx * c = (b200_buffer_ctx *)buffer->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
     B200_CUDA_CHECK(cudaMemcpyAsync(dst->data, src->data, b200_alloc_size(src), cudaMemcpyDeviceToDevice, cudaStreamPerThread));
@@ -186,12 +207,12 @@ GGML_CALL static void b200_backend_synchronize(ggml_backend_t b) {
 // the synchronous buffer path (they are re-laid-out on upload)
 GGML_CALL static void b200_backend_set_tensor_async(ggml_backend_t b, ggml_tensor * t, const void * data, size_t off, size_t size) {
     b200_backend_ctx * c = (b200_backend_ctx *)b->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
-    if (b200_tensor_is_repacked(t)) { B200_CUDA_CHECK(cudaStreamSynchronize(c->stream)); t->buffer->iface.set_tensor(t->buffer, t, data, off, size); return; }
+    if (b200_wire_staged(t)) { B200_CUDA_CHECK(cudaStreamSynchronize(c->stream)); b200_buffer_set_tensor(t->view_src ? t->view_src->buffer : t->buffer, t, data, off, size); return; }
     B200_CUDA_CHECK(cudaMemcpyAsync((char *)t->data + off, data, size, cudaMemcpyHostToDevice, c->stream));
 }
 GGML_CALL static void b200_backend_get_tensor_async(ggml_backend_t b, const ggml_tensor * t, void * data, size_t off, size_t size) {
     b200_backend_ctx * c = (b200_backend_ctx *)b->context; B200_CUDA_CHECK(cudaSetDevice(c->device));
-    if (b200_tensor_is_repacked(t)) { B200_CUDA_CHECK(cudaStreamSynchronize(c->stream)); t->buffer->iface.get_tensor(t->buffer, t, data, off, size); return; }
+    if (b200_wire_staged(t)) { B200_CUDA_CHECK(cudaStreamSynchronize(c->stream)); b200_buffer_get_tensor(t->view_src ? t->view_src->buffer : t->buffer, t, data, off, size); return; }
     B200_CUDA_CHECK(cudaMemcpyAsync(data, (const char *)t->data + off, size, cudaMemcpyDeviceToHost, c->stream));
 }
 GGML_CALL static bool b200_backend_cpy_tensor_async(ggml_backend_t bsrc, ggml_backend_t bdst, const ggml_tensor * src, ggml_tensor * dst) {
@@ -242,6 +263,12 @@ static bool b200_can_mul_mat(const ggml_tensor * w, const ggml_tensor * x, const
     if (!(w->ne[2] == 1 || (w->ne[2] == x->ne[2] && x->ne[3] == 1))) return false;
     return true;
 }
+// MoE expert ids: int32 [n_used, n_tokens], consecutive within a token.  The tokens' rows may lie further apart: ggml_top_k returns a view of the
+// argsort result (nb1 = n_expert * 4), and the scheduler's copy keeps that layout; graph_compute gathers such rows into its workspace.
+static bool b200_ids_ok(const ggml_tensor * ids) {
+    return ids->type == GGML_TYPE_I32 && ids->nb[0] == sizeof(int32_t) && ids->nb[1] >= ids->ne[0] * sizeof(int32_t) && ids->ne[2] == 1 && ids->ne[3] == 1;
+}
+static bool b200_ids_strided(const ggml_tensor * ids) { return ids->ne[1] > 1 && ids->nb[1] != ids->ne[0] * sizeof(int32_t); }
 GGML_CALL static bool b200_backend_supports_op(ggml_backend_t, const ggml_tensor * op) {
     switch (op->op) {
         case GGML_OP_NONE: case GGML_OP_RESHAPE: case GGML_OP_VIEW: case GGML_OP_PERMUTE: case GGML_OP_TRANSPOSE: return true;
@@ -256,7 +283,7 @@ GGML_CALL static bool b200_backend_supports_op(ggml_backend_t, const ggml_tensor
             const bool ug = op->op == GGML_OP_MOE_FUSED_UP_GATE;
             const ggml_tensor * w = op->src[0]; const ggml_tensor * g = ug ? op->src[1] : nullptr; const ggml_tensor * x = op->src[ug ? 2 : 1]; const ggml_tensor * ids = op->src[ug ? 3 : 2];
             if (!w || !x || !ids || (ug && (!g || g->type != w->type || !ggml_are_same_shape(g, w) || op->src[4] || op->src[5] || b200_unary(b200_op_param_i32(op, 0)) < 0))) return false;
-            if (!b200_weight_ok(w) || (g && !b200_weight_ok(g)) || x->type != GGML_TYPE_F32 || !ggml_is_contiguous(x) || ids->type != GGML_TYPE_I32 || !ggml_is_contiguous(ids)) return false;
+            if (!b200_weight_ok(w) || (g && !b200_weight_ok(g)) || x->type != GGML_TYPE_F32 || !ggml_is_contiguous(x) || !b200_ids_ok(ids)) return false;
             if (op->type != GGML_TYPE_F32 || !ggml_is_contiguous(op) || w->ne[0] != x->ne[0] || x->ne[3] != 1 || ids->ne[1] != x->ne[2] || ids->ne[0] % x->ne[1]) return false;
             return x->ne[1] * (w->ne[0] + w->ne[0] / 4) <= 200 * 1024;      // one token's columns must fit
         }
@@ -341,7 +368,14 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
                 // prefill batches: grouped GEMM over expert-sorted slots (routing on the device); small batches: the mat-vec kernel
                 const size_t need = b200q_mul_mat_id_workspace(w->type, w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], (int)w->ne[2], ug);
                 void * ws = need ? c->workspace(need) : nullptr;
-                B200Q_CHECK(b200q_mul_mat_id(w->type, w->data, g ? g->data : nullptr, (int)w->ne[2], (const int32_t *)ids->data, (const float *)x->data, (float *)node->data,
+                const int32_t * id = (const int32_t *)ids->data;
+                if (b200_ids_strided(ids)) {    // strided ids (ggml_top_k): gathered into a contiguous tail of the workspace, on the stream (capture-safe)
+                    const size_t row = ids->ne[0] * sizeof(int32_t), tail = (need + 255) & ~(size_t)255;
+                    char * base = (char *)c->workspace(tail + row * ids->ne[1]);
+                    B200_CUDA_CHECK(cudaMemcpy2DAsync(base + tail, row, ids->data, ids->nb[1], row, ids->ne[1], cudaMemcpyDeviceToDevice, c->stream));
+                    ws = need ? base : nullptr; id = (const int32_t *)(base + tail);
+                }
+                B200Q_CHECK(b200q_mul_mat_id(w->type, w->data, g ? g->data : nullptr, (int)w->ne[2], id, (const float *)x->data, (float *)node->data,
                                              w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], ug ? b200_unary(b200_op_param_i32(node, 0)) : 0, limit,
                                              ws, need, c->stream));
             } break;

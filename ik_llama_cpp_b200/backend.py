@@ -339,6 +339,33 @@ def mul_mat_id_dispatch(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gat
     return dst
 
 
+def moe_up_gate_merged_workspace(w: ExpertTensor, n_tokens: int, n_used: int, nb1: int) -> int:
+    """Bytes of device workspace moe_up_gate_merged needs (w: merged experts, m = 2 n_ff); 0 exactly when it takes the mat-vec path."""
+    assert w.m % 2 == 0
+    return int(_lib.lib().b200q_moe_up_gate_merged_workspace(w.ggml_type, w.m // 2, w.k, n_used, nb1, n_tokens, w.n_expert))
+
+
+def moe_up_gate_merged(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, unary: str = "silu", limit: float = 0.0,
+                       out: torch.Tensor | None = None) -> torch.Tensor:
+    """GGML_OP_MOE_FUSED_UP_GATE over merged up/gate experts (ffn_gate_up_exps, src[1] = NULL): w holds n_expert matrices [2 n_ff x K] whose rows
+    [0, n_ff) are the gate and [n_ff, 2 n_ff) the up rows.  x f32 [n_tokens, nb1, K], ids int32 [n_tokens, n_used] -> dst f32 [n_tokens, n_used, n_ff],
+    dst[t, e] = unary(gate[id] . x[t, e % nb1]) * (up[id] . x[t, e % nb1]).  The grouped GEMM above the crossover of mul_mat_id_dispatch, the mat-vec
+    kernel below it."""
+    _require_cuda()
+    n_tokens, nb1, n_used = _mul_mat_id_args(w, x, ids, None)
+    assert w.m % 2 == 0, "merged up/gate experts have 2 n_ff rows"
+    n_ff = w.m // 2
+    dst = out if out is not None else torch.empty((n_tokens, n_used, n_ff), dtype=torch.float32, device=x.device)
+    assert dst.shape == (n_tokens, n_used, n_ff) and dst.dtype == torch.float32 and dst.is_contiguous()
+    need = moe_up_gate_merged_workspace(w, n_tokens, n_used, nb1)
+    ws = _workspace(need, x.device) if need else None
+    with torch.cuda.device(x.device):
+        check(_lib.lib().b200q_moe_up_gate_merged(w.ggml_type, w.ptr, w.n_expert, ids.data_ptr(), x.data_ptr(), dst.data_ptr(), n_ff, w.k, n_used, nb1,
+                                                  n_tokens, UNARY[unary], float(limit), ws.data_ptr() if ws is not None else None,
+                                                  ws.numel() if ws is not None else 0, _stream()), "b200q_moe_up_gate_merged")
+    return dst
+
+
 def dequantize_bf16(w: QuantTensor) -> torch.Tensor:
     _require_cuda()
     out = torch.empty((w.m, w.k), dtype=torch.bfloat16, device=w.planes.device)

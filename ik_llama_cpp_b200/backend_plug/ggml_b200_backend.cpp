@@ -279,10 +279,14 @@ GGML_CALL static bool b200_backend_supports_op(ggml_backend_t, const ggml_tensor
                    op->src[1]->ne[0] == op->ne[0] && (ggml_nelements(op->src[1]) == op->ne[0] || ggml_are_same_shape(op, op->src[1]));
         case GGML_OP_MUL_MAT_ID: case GGML_OP_MOE_FUSED_UP_GATE: {
             // MoE: expert ids resolved on the device; prefill batches take the grouped GEMM, small ones the mat-vec kernel (walked in token chunks
-            // when a batch exceeds the shared-memory capacity of one launch)
+            // when a batch exceeds the shared-memory capacity of one launch).  Up/gate experts either split (src[1] = gate) or merged (src[1] = NULL:
+            // ffn_gate_up_exps [K, 2 n_ff, E], gate rows first); biased forms (src[4], src[5]) stay on the CPU
             const bool ug = op->op == GGML_OP_MOE_FUSED_UP_GATE;
             const ggml_tensor * w = op->src[0]; const ggml_tensor * g = ug ? op->src[1] : nullptr; const ggml_tensor * x = op->src[ug ? 2 : 1]; const ggml_tensor * ids = op->src[ug ? 3 : 2];
-            if (!w || !x || !ids || (ug && (!g || g->type != w->type || !ggml_are_same_shape(g, w) || op->src[4] || op->src[5] || b200_unary(b200_op_param_i32(op, 0)) < 0))) return false;
+            if (!w || !x || !ids || (ug && (op->src[4] || op->src[5] || b200_unary(b200_op_param_i32(op, 0)) < 0))) return false;
+            if (g && (g->type != w->type || !ggml_are_same_shape(g, w))) return false;
+            // merged: [gate; up] with n_ff rows each, n_ff a valid row count of the type (a multiple of 4 for the _R4 types)
+            if (ug && !g && (w->ne[1] != 2 * op->ne[0] || b200q_plane_bytes(w->type, op->ne[0], w->ne[0]) <= 0)) return false;
             if (!b200_weight_ok(w) || (g && !b200_weight_ok(g)) || x->type != GGML_TYPE_F32 || !ggml_is_contiguous(x) || !b200_ids_ok(ids)) return false;
             if (op->type != GGML_TYPE_F32 || !ggml_is_contiguous(op) || w->ne[0] != x->ne[0] || x->ne[3] != 1 || ids->ne[1] != x->ne[2] || ids->ne[0] % x->ne[1]) return false;
             return x->ne[1] * (w->ne[0] + w->ne[0] / 4) <= 200 * 1024;      // one token's columns must fit
@@ -365,8 +369,10 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
                 const bool ug = node->op == GGML_OP_MOE_FUSED_UP_GATE;
                 const ggml_tensor * w = node->src[0]; const ggml_tensor * g = ug ? node->src[1] : nullptr; const ggml_tensor * x = node->src[ug ? 2 : 1]; const ggml_tensor * ids = node->src[ug ? 3 : 2];
                 float limit = 0.0f; if (ug) memcpy(&limit, (const char *)node->op_params + sizeof(int32_t), sizeof(float));
+                const bool merged = ug && !g;       // ffn_gate_up_exps: node->ne[0] = n_ff gate rows, then n_ff up rows per expert
                 // prefill batches: grouped GEMM over expert-sorted slots (routing on the device); small batches: the mat-vec kernel
-                const size_t need = b200q_mul_mat_id_workspace(w->type, w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], (int)w->ne[2], ug);
+                const size_t need = merged ? b200q_moe_up_gate_merged_workspace(w->type, node->ne[0], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], (int)w->ne[2])
+                                           : b200q_mul_mat_id_workspace(w->type, w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], (int)w->ne[2], ug);
                 void * ws = need ? c->workspace(need) : nullptr;
                 const int32_t * id = (const int32_t *)ids->data;
                 if (b200_ids_strided(ids)) {    // strided ids (ggml_top_k): gathered into a contiguous tail of the workspace, on the stream (capture-safe)
@@ -375,9 +381,11 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
                     B200_CUDA_CHECK(cudaMemcpy2DAsync(base + tail, row, ids->data, ids->nb[1], row, ids->ne[1], cudaMemcpyDeviceToDevice, c->stream));
                     ws = need ? base : nullptr; id = (const int32_t *)(base + tail);
                 }
-                B200Q_CHECK(b200q_mul_mat_id(w->type, w->data, g ? g->data : nullptr, (int)w->ne[2], id, (const float *)x->data, (float *)node->data,
-                                             w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], ug ? b200_unary(b200_op_param_i32(node, 0)) : 0, limit,
-                                             ws, need, c->stream));
+                const int unary = ug ? b200_unary(b200_op_param_i32(node, 0)) : 0;
+                if (merged) B200Q_CHECK(b200q_moe_up_gate_merged(w->type, w->data, (int)w->ne[2], id, (const float *)x->data, (float *)node->data,
+                                                                 node->ne[0], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], unary, limit, ws, need, c->stream));
+                else B200Q_CHECK(b200q_mul_mat_id(w->type, w->data, g ? g->data : nullptr, (int)w->ne[2], id, (const float *)x->data, (float *)node->data,
+                                                  w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], unary, limit, ws, need, c->stream));
             } break;
             case GGML_OP_FUSED_UP_GATE: {
                 const ggml_tensor * up = node->src[0]; const ggml_tensor * gate = node->src[1]; const ggml_tensor * x = node->src[2];

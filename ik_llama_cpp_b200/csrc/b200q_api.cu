@@ -377,29 +377,41 @@ int b200q_add_rows(const float * a, const float * b, float * dst, int64_t m, int
     if (!a || !b || !dst) return fail(B200Q_E_ARG, "b200q_add_rows: bad argument");
     return check_launch(b200q_launch_add_rows(a, b, dst, m, n, nb, (cudaStream_t)stream), "b200q_add_rows");
 }
-int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
-                         int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream) {
-    if (!W || !ids || !x || !dst || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_vec: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_id_vec: no CUDA device");
-    if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_mul_mat_id_vec: activations must be 16-byte aligned");
-    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_vec: bad token / slot counts");
+/* The MoE entry points share one body per path.  An operand is a (tensor, row origin) pair inside expert matrices of rows_layout rows
+ * (b200q_mmvq_id_desc): the split up/gate form passes origin 0 and rows_layout = m, merged [gate; up] experts pass one tensor twice with
+ * rows_layout = 2 m, up at row m and gate at row 0. */
+struct moe_operands { const void * W; const void * W_gate; int64_t rows_layout, W_row0, gate_row0; };
+static void moe_desc(b200q_mmvq_id_desc & d, int type, const moe_operands & o, int n_expert, int64_t m, int64_t k, int n_used, int nb1, int unary, float limit) {
+    memset(&d, 0, sizeof d);
+    d.type = type; d.W = o.W; d.W2 = o.W_gate; d.rows_layout = o.rows_layout; d.W_row0 = o.W_row0; d.W2_row0 = o.gate_row0;
+    d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.act = unary; d.limit = limit;
+}
+static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst,
+                   int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream, const char * what) {
+    if (!o.W || !ids || !x || !dst || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
+    if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "%s: activations must be 16-byte aligned", what);
+    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
     // the quantised activation columns of a launch live in shared memory: larger batches are walked in token chunks (same kernel, the expert ids
     // never leave the device).  Prefill batches are served by the grouped GEMM (b200q_mul_mat_id_gemm) once b200q_mul_mat_id selects it.
     const int64_t col_bytes = (int64_t)nb1 * (k + k / 4);
     int chunk = (int)((200 * 1024) / (col_bytes > 0 ? col_bytes : 1));
     static const int forced = [] { const char * e = getenv("B200Q_MOE_CHUNK_TOKENS"); return e ? atoi(e) : 0; }();
     if (forced > 0 && forced < chunk) chunk = forced;
-    if (chunk < 1) return fail(B200Q_E_SHAPE, "b200q_mul_mat_id_vec: one token's activation columns do not fit shared memory");
+    if (chunk < 1) return fail(B200Q_E_SHAPE, "%s: one token's activation columns do not fit shared memory", what);
     for (int t0 = 0; t0 < n_tokens; t0 += chunk) {
         const int nt = n_tokens - t0 < chunk ? n_tokens - t0 : chunk;
-        b200q_mmvq_id_desc d; memset(&d, 0, sizeof d);
-        d.type = type; d.W = W; d.W2 = W_gate; d.ids = ids + (int64_t)t0 * n_used; d.x = x + (int64_t)t0 * nb1 * k; d.dst = dst + (int64_t)t0 * n_used * m;
-        d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.n_tokens = nt;
-        d.act = unary; d.limit = limit; d.sm_count = di.sm_count; d.pdl = opt_pdl();
-        const int rc = check_launch(b200q_launch_mmvq_id(d, (cudaStream_t)stream), "b200q_mul_mat_id_vec");
+        b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
+        d.ids = ids + (int64_t)t0 * n_used; d.x = x + (int64_t)t0 * nb1 * k; d.dst = dst + (int64_t)t0 * n_used * m; d.n_tokens = nt;
+        d.sm_count = di.sm_count; d.pdl = opt_pdl();
+        const int rc = check_launch(b200q_launch_mmvq_id(d, (cudaStream_t)stream), what);
         if (rc) return rc;
     }
     return B200Q_OK;
+}
+int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
+                         int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream) {
+    return moe_vec(type, {W, W_gate, m, 0, 0}, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, stream, "b200q_mul_mat_id_vec");
 }
 
 /* MoE prefill: grouped wgmma GEMM over expert-sorted slots (b200q_moe.cu), versus the mat-vec kernel, which needs no routing or gather pass.
@@ -408,32 +420,60 @@ int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_ex
  *  - MOE_FUSED_UP_GATE follows the average rows per expert, n_slots / n_expert: at 4 rows Mixtral is still 0.82x while the others are 1.3-1.45x,
  *    at 6 rows every shape is 1.4-2.2x faster on the grouped path.  Grouped when n_slots > 5 * n_expert.
  *  - MUL_MAT_ID follows the number of slots, whatever the expert count: 24 slots 0.84x (Mixtral), 32 slots 0.94-1.08x, 64 slots 1.18-2.3x on
- *    every shape.  Grouped when n_slots > 32. */
+ *    every shape.  Grouped when n_slots > 32.
+ * Merged up/gate experts run the same launches on the same bytes as the split form, so they share its crossover. */
 static constexpr int64_t MOE_UP_GATE_MIN_ROWS_PER_EXPERT = 5;
 static constexpr int64_t MOE_MUL_MAT_ID_MIN_SLOTS = 32;
-size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate) {
+static size_t moe_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate, int64_t rows_layout) {
     if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate)) return 0;
     const int64_t n_slots = (int64_t)n_tokens * n_used;
     if (up_gate ? n_slots <= MOE_UP_GATE_MIN_ROWS_PER_EXPERT * n_expert : n_slots <= MOE_MUL_MAT_ID_MIN_SLOTS) return 0;
-    return b200q_moe_gemm_workspace_bytes(type, m, k, n_slots, n_expert, up_gate);
+    return b200q_moe_gemm_workspace_bytes(type, m, k, n_slots, n_expert, up_gate, rows_layout);
+}
+size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate) {
+    return moe_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate, m);
+}
+static int moe_gemm(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst, int64_t m, int64_t k,
+                    int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream, const char * what) {
+    if (!o.W || !ids || !x || !dst || !workspace || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
+    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
+    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, o.W_gate != nullptr))
+        return fail(B200Q_E_SHAPE, "%s: shape not supported by the grouped GEMM (K %% 256, n_expert <= 1024, type)", what);
+    b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
+    d.ids = ids; d.x = x; d.dst = dst; d.n_tokens = n_tokens; d.sm_count = di.sm_count;
+    return check_launch(b200q_launch_moe_gemm(d, workspace, workspace_bytes, (cudaStream_t)stream), what);
 }
 int b200q_mul_mat_id_gemm(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
                           int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
-    if (!W || !ids || !x || !dst || !workspace || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_gemm: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_id_gemm: no CUDA device");
-    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "b200q_mul_mat_id_gemm: bad token / slot counts");
-    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, W_gate != nullptr))
-        return fail(B200Q_E_SHAPE, "b200q_mul_mat_id_gemm: shape not supported by the grouped GEMM (K %% 256, n_expert <= 1024, type)");
-    b200q_mmvq_id_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.W = W; d.W2 = W_gate; d.ids = ids; d.x = x; d.dst = dst; d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.n_tokens = n_tokens;
-    d.act = unary; d.limit = limit; d.sm_count = di.sm_count;
-    return check_launch(b200q_launch_moe_gemm(d, workspace, workspace_bytes, (cudaStream_t)stream), "b200q_mul_mat_id_gemm");
+    return moe_gemm(type, {W, W_gate, m, 0, 0}, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, workspace, workspace_bytes, stream,
+                    "b200q_mul_mat_id_gemm");
 }
 int b200q_mul_mat_id(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
                      int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
     if (b200q_mul_mat_id_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, W_gate != nullptr) == 0)
         return b200q_mul_mat_id_vec(type, W, W_gate, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, stream);
     return b200q_mul_mat_id_gemm(type, W, W_gate, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, workspace, workspace_bytes, stream);
+}
+
+/* MOE_FUSED_UP_GATE over merged experts: W_gate_up holds n_expert matrices [2 m x k], gate rows [0, m) then up rows [m, 2 m) */
+size_t b200q_moe_up_gate_merged_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert) {
+    if (m < 1 || m > INT32_MAX / 4) return 0;
+    return moe_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, 1, 2 * m);
+}
+int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_expert, const int32_t * ids, const float * x, float * dst,
+                             int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
+    static const char * what = "b200q_moe_up_gate_merged";
+    if (!W_gate_up || m < 1 || m > INT32_MAX / 4) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    b200q_layout L;
+    if (const int rc = b200q_make_layout(type, 2 * m, k, &L)) return rc == -1 ? fail(B200Q_E_TYPE, "%s: unsupported ggml type", what)
+                                                                             : fail(B200Q_E_SHAPE, "%s: k = %lld is not a multiple of the type's block", what, (long long)k);
+    if (L.wire > 1 && m % L.wire)
+        return fail(B200Q_E_SHAPE, "%s: m = %lld must be a multiple of %d for this type (its rows are interleaved in groups of %d)", what, (long long)m, L.wire, L.wire);
+    const moe_operands o{W_gate_up, W_gate_up, 2 * m, m, 0};
+    if (b200q_moe_up_gate_merged_workspace(type, m, k, n_used, nb1, n_tokens, n_expert) == 0)
+        return moe_vec(type, o, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, stream, what);
+    return moe_gemm(type, o, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, workspace, workspace_bytes, stream, what);
 }
 int b200q_mul_mat_host(int type, const void * W, const float * x_host, float * dst_host, int64_t m, int64_t k, int64_t n, void * stream) {
     cudaStream_t st = (cudaStream_t)stream; cudaError_t e; int rc;

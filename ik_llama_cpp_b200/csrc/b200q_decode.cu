@@ -163,13 +163,15 @@ int b200q_launch_mmvq(const b200q_mmvq_desc & d, cudaStream_t st) {
     }
 }
 
-// MoE decode (GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE, small batches): see k_mmvq_id / k_wire_mmvq_id
+// MoE decode (GGML_OP_MUL_MAT_ID / MOE_FUSED_UP_GATE, small batches): see k_mmvq_id / k_wire_mmvq_id.  The operands' row origins are folded into
+// the plane pointers here (b200q_planes_at): the kernels see the rows [row0, row0 + M) of each expert as an [M x K] matrix, estride bytes apart.
 int b200q_launch_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
     if (d.n_tokens < 1 || d.n_used < 1 || d.nb1 < 1 || d.n_used % d.nb1 || d.n_expert < 1 || !d.W || !d.ids || !d.x || !d.dst) return -2;
+    if (d.M < 1 || d.W_row0 < 0 || d.W2_row0 < 0 || d.W_row0 + d.M > d.rows_layout || (d.W2 && d.W2_row0 + d.M > d.rows_layout)) return -2;
     if (b200q_is_wire_type(d.type)) return b200q_launch_wire_mmvq_id(d, st);
-    b200q_layout L; const int rc = b200q_make_layout(d.type, d.M, d.K, &L); if (rc) return rc;
+    b200q_layout L; const int rc = b200q_make_layout(d.type, d.rows_layout, d.K, &L); if (rc) return rc;
     mmvq_id_args a; memset(&a, 0, sizeof a);
-    a.P = b200q_planes_from((const uint8_t *)d.W, L); if (d.W2) a.P2 = b200q_planes_from((const uint8_t *)d.W2, L);
+    a.P = b200q_planes_at((const uint8_t *)d.W, L, d.W_row0); if (d.W2) a.P2 = b200q_planes_at((const uint8_t *)d.W2, L, d.W2_row0);
     a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used; a.n_used = d.n_used; a.nb1 = d.nb1; a.ncx = d.n_tokens * d.nb1;
     a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit;
     switch (d.type) {

@@ -690,13 +690,14 @@ template <int BN, bool GROUPED> unsigned row_tiles(int64_t N, int64_t n_mat) {
     return (unsigned)((N + BN - 1) / BN + (GROUPED ? std::min<int64_t>(n_mat, N) : 0));
 }
 
-// dst f32 [N][M] = A bf16 [M][K] x B bf16 [N][K]; GROUPED: A holds n_mat experts [n_mat][M][K], those of rt.e0 .. rt.e1-1
+// dst f32 [N][M] = A bf16 [M][K] x B bf16 [N][K]; GROUPED: A holds n_mat experts [n_mat][a_rows][K], those of rt.e0 .. rt.e1-1, and the product
+// reads the first M rows of each (A_bf16 may point at a later row of expert 0: a row range of every expert)
 template <int BN, bool GROUPED>
-int launch_gemm_bf16(const void * A_bf16, int64_t n_mat, const void * B_bf16, float * dst, int64_t M, int64_t N, int64_t K, int k_split,
+int launch_gemm_bf16(const void * A_bf16, int64_t n_mat, int64_t a_rows, const void * B_bf16, float * dst, int64_t M, int64_t N, int64_t K, int k_split,
                      const b200q_moe_route & rt, cudaStream_t st) {
     using cfg = gemm_cfg<BN>;
     CUtensorMap tmA, tmB;
-    if (make_tmap(&tmA, TM_BF16, GROUPED ? 3 : 2, A_bf16, {K, M, n_mat}, {K * 2, M * K * 2}, {64, BM, 1}, true)) return -10;
+    if (make_tmap(&tmA, TM_BF16, GROUPED ? 3 : 2, A_bf16, {K, M, n_mat}, {K * 2, a_rows * K * 2}, {64, BM, 1}, true)) return -10;
     if (make_tmap(&tmB, TM_BF16, 2, B_bf16, {K, N}, {K * 2}, {64, BN}, true)) return -11;
     if (int rc = opt_in_smem((const void *)k_gemm_bf16<BN, GROUPED>, cfg::SMEM)) return rc;
     dim3 grid((unsigned)((M + BM - 1) / BM), row_tiles<BN, GROUPED>(N, n_mat), (unsigned)k_split);
@@ -716,18 +717,20 @@ constexpr bool gemmq_supported(int type) {
 }
 
 // k_gemm_q over the segments of d.  GROUPED: d.W[i] holds n_mat expert matrices (one 3-D map per plane covers them all) and blockIdx.y walks
-// the tile table of rt
+// the tile table of rt.  rows: when not null, segment i is the row range [rows->row0[i], rows->row0[i] + d.M[i]) of matrices of rows->rows_layout
+// rows (merged up/gate experts): its maps start at that row and end after d.M[i] rows, so a partial last tile is zero-filled, not the next range
 template <int TYPE, int NB, bool GROUPED>
-int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, cudaStream_t st) {
+int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, const b200q_moe_gemm * rows, cudaStream_t st) {
     using cfg = typename gemmq_policy<TYPE, NB, GROUPED>::cfg;
     gemm_decode_args<cfg::N_PLANES> a; memset(&a, 0, sizeof a);
     const int box[3] = {128, cfg::P1, cfg::P2};                   // bytes per row of each plane per 256 weights
     int tiles = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        b200q_layout L; if (b200q_make_layout(TYPE, d.M[i], d.K, &L)) return -1;
+        b200q_layout L; if (b200q_make_layout(TYPE, rows ? rows->rows_layout : d.M[i], d.K, &L)) return -1;
         for (int p = 0; p < cfg::N_PLANES; ++p) {
             const int64_t row_bytes = (d.K / 256) * box[p];
-            if (make_tmap(&a.tmP[p][i], TM_U8, GROUPED ? 3 : 2, (const char *)d.W[i] + L.plane_off[p], {row_bytes, d.M[i], n_mat},
+            const char * base = (const char *)d.W[i] + L.plane_off[p] + (rows ? b200q_row_offset(L, p, rows->row0[i]) : 0);
+            if (make_tmap(&a.tmP[p][i], TM_U8, GROUPED ? 3 : 2, base, {row_bytes, d.M[i], n_mat},
                                     {row_bytes, L.total_bytes}, {box[p], BM, 1}, p == 0)) return p == 0 ? -10 : -13;
         }
         a.seg[i].dst = d.dst[i]; a.seg[i].M = (int)d.M[i]; a.seg[i].tile0 = tiles;
@@ -741,9 +744,10 @@ int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const 
     return (int)cudaGetLastError();
 }
 template <bool GROUPED>
-int launch_gemm_q(int type, bool bn256, const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, cudaStream_t st) {
+int launch_gemm_q(int type, bool bn256, const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, const b200q_moe_gemm * rows,
+                  cudaStream_t st) {
     switch (type) {
-#define X(T) case T: return bn256 ? launch_gemm_q<T, 1, GROUPED>(d, k_split, n_mat, rt, st) : launch_gemm_q<T, 0, GROUPED>(d, k_split, n_mat, rt, st);
+#define X(T) case T: return bn256 ? launch_gemm_q<T, 1, GROUPED>(d, k_split, n_mat, rt, rows, st) : launch_gemm_q<T, 0, GROUPED>(d, k_split, n_mat, rt, rows, st);
         GEMMQ_TYPES(X)
 #undef X
         default: return -1;
@@ -857,7 +861,7 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         const int64_t tiles = mt * ((N + bn - 1) / bn);
         const int k_split = gemmq_choose_split(tiles, K / 256, sm_count);
         if (k_split > 1) for (int i = 0; i < d.n_seg; ++i) { cudaError_t e = cudaMemsetAsync(d.dst[i], 0, (size_t)d.M[i] * N * sizeof(float), st); if (e != cudaSuccess) return -3; }
-        return launch_gemm_q<false>(type, bn256, d, k_split, 1, b200q_moe_route{}, st);
+        return launch_gemm_q<false>(type, bn256, d, k_split, 1, b200q_moe_route{}, nullptr, st);
     }
     // unfused: bf16 weight scratch + plain bf16 GEMM per tensor; tile / split selection: fill ~1 wave of the SMs
     for (int i = 0; i < d.n_seg; ++i) {
@@ -872,8 +876,8 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         if (k_split > 1) { cudaError_t e = cudaMemsetAsync(d.dst[i], 0, (size_t)M * N * sizeof(float), st); if (e != cudaSuccess) return -3; }
         if (ws_bytes < (size_t)b200q_align_up(M * K * 2, 256)) return -5;
         int rc = b200q_launch_dequant_bf16(d.W[i], L, wscratch, st); if (rc) return rc;
-        rc = bn256 ? launch_gemm_bf16<256, false>(wscratch, 1, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st)
-                   : launch_gemm_bf16<128, false>(wscratch, 1, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st);
+        rc = bn256 ? launch_gemm_bf16<256, false>(wscratch, 1, M, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st)
+                   : launch_gemm_bf16<128, false>(wscratch, 1, M, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st);
         if (rc) return rc;
     }
     return 0;
@@ -891,26 +895,30 @@ int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, void * o
 
 // MoE grouped GEMM over the expert-sorted rows g.xb.  Types of the fused kernel: ONE launch over the row tiles of the segments, the weights
 // decoded inside the kernel.  Every other type: the experts are walked in groups whose bf16 copies fit `wscratch` (a contiguous range of the
-// sorted rows each); per group and segment the experts that received rows are dequantised, then one grouped bf16 GEMM.
+// sorted rows each); per group and segment the experts that received rows are dequantised, then one grouped bf16 GEMM.  Segment i reads the rows
+// [g.row0[i], g.row0[i] + g.M) of matrices of g.rows_layout rows; segments of one tensor (merged up/gate experts) share one dequantised copy.
 int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t ws_bytes, cudaStream_t st) {
     if (g.K % 256 || g.n_seg < 1 || g.n_seg > 2 || g.n_rows < 1 || (g.bn != 128 && g.bn != 256)) return -2;
+    for (int i = 0; i < g.n_seg; ++i) if (g.row0[i] < 0 || g.row0[i] + g.M > g.rows_layout) return -2;
     const bool bn256 = g.bn == 256;
     if (gemmq_supported(g.type)) {
         b200q_gemm_multi d; memset(&d, 0, sizeof d);
         d.type = g.type; d.n_seg = g.n_seg; d.K = g.K; d.N = g.n_rows; d.xb = g.xb;
         for (int i = 0; i < g.n_seg; ++i) { d.W[i] = g.W[i]; d.dst[i] = g.dst[i]; d.M[i] = g.M; }
-        return launch_gemm_q<true>(g.type, bn256, d, 1, g.n_expert, g.rt, st);
+        return launch_gemm_q<true>(g.type, bn256, d, 1, g.n_expert, g.rt, &g, st);
     }
-    b200q_layout L; if (b200q_make_layout(g.type, g.M, g.K, &L)) return -1;
-    const int64_t ebytes = g.M * g.K * 2;
+    b200q_layout L; if (b200q_make_layout(g.type, g.rows_layout, g.K, &L)) return -1;
+    const int64_t ebytes = g.rows_layout * g.K * 2;
     const int64_t per = std::min<int64_t>(g.n_expert, (int64_t)(ws_bytes / (size_t)ebytes));
     if (per < 1) return -5;
     for (int e0 = 0; e0 < g.n_expert; e0 += (int)per) {
         b200q_moe_route rt = g.rt; rt.e0 = e0; rt.e1 = (int)std::min<int64_t>(g.n_expert, e0 + per);
         for (int i = 0; i < g.n_seg; ++i) {
-            int rc = b200q_launch_dequant_bf16_experts(g.W[i], L, wscratch, rt.e0, rt.e1 - rt.e0, g.rt.bounds, st); if (rc) return rc;
-            rc = bn256 ? launch_gemm_bf16<256, true>(wscratch, rt.e1 - rt.e0, g.xb, g.dst[i], g.M, g.n_rows, g.K, 1, rt, st)
-                       : launch_gemm_bf16<128, true>(wscratch, rt.e1 - rt.e0, g.xb, g.dst[i], g.M, g.n_rows, g.K, 1, rt, st);
+            int rc = 0;
+            if (i == 0 || g.W[i] != g.W[i - 1]) { rc = b200q_launch_dequant_bf16_experts(g.W[i], L, wscratch, rt.e0, rt.e1 - rt.e0, g.rt.bounds, st); if (rc) return rc; }
+            const char * A = (const char *)wscratch + g.row0[i] * g.K * 2;
+            rc = bn256 ? launch_gemm_bf16<256, true>(A, rt.e1 - rt.e0, g.rows_layout, g.xb, g.dst[i], g.M, g.n_rows, g.K, 1, rt, st)
+                       : launch_gemm_bf16<128, true>(A, rt.e1 - rt.e0, g.rows_layout, g.xb, g.dst[i], g.M, g.n_rows, g.K, 1, rt, st);
             if (rc) return rc;
         }
     }

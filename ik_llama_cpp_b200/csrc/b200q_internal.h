@@ -72,10 +72,13 @@ static inline size_t b200q_q8_image_bytes(int64_t k) { return (size_t)(k + 12 * 
 int b200q_launch_repack(const void * wire, void * planes, const b200q_layout & L, int inverse, cudaStream_t st);
 int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out, cudaStream_t st);
 int b200q_launch_mmvq(const b200q_mmvq_desc & d, cudaStream_t st);
-// MoE decode: W = n_expert matrices [M x K], b200q_plane_bytes(type, M, K) apart; ids device int32 [n_tokens][n_used]; x f32 [n_tokens][nb1][K]; dst f32 [n_tokens][n_used][M]
+// MoE decode: W = n_expert matrices [rows_layout x K], b200q_plane_bytes(type, rows_layout, K) apart; ids device int32 [n_tokens][n_used];
+// x f32 [n_tokens][nb1][K]; dst f32 [n_tokens][n_used][M].  An operand is rows [row0, row0 + M) of its expert matrices: the split form is
+// W_row0 = W2_row0 = 0 with rows_layout = M, merged up/gate experts ([gate; up], rows_layout = 2 M) are W = W2 with W_row0 = M (up), W2_row0 = 0 (gate).
 struct b200q_mmvq_id_desc {
     int type; const void * W; const void * W2; const int32_t * ids; const float * x; float * dst;
     int64_t M, K; int n_expert, n_used, nb1, n_tokens; int act; float limit; int sm_count; int pdl;
+    int64_t rows_layout, W_row0, W2_row0;
 };
 int b200q_launch_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
 int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
@@ -106,7 +109,8 @@ int b200q_gemm_fused_type(int type);
 //   tiles[tile_start[e] .. tile_start[e+1]): {e, first sorted row} of expert e's tiles of BN rows;  e0 .. e1: the experts a launch covers.
 struct b200q_moe_route { const int * bounds; const int * tile_start; const int2 * tiles; const int * slot; int e0, e1; };
 struct b200q_moe_gemm {
-    int type; int n_seg; const void * W[2]; float * dst[2];   // n_expert matrices [M x K] per segment, b200q_plane_bytes apart; dst f32 [slot][M]
+    int type; int n_seg; const void * W[2]; float * dst[2];   // n_expert matrices [rows_layout x K] per segment, b200q_plane_bytes apart; dst f32 [slot][M]
+    int64_t row0[2], rows_layout;                             // segment i reads rows [row0[i], row0[i] + M) of its matrices (see b200q_mmvq_id_desc)
     int64_t M, K; int n_expert; int64_t n_rows;               // n_rows: rows of xb = number of slots (the routed rows are a prefix)
     const void * xb; int bn;                                   // bf16 [n_rows][K] in expert-sorted order; tile width (128 / 256)
     b200q_moe_route rt;
@@ -118,5 +122,18 @@ int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t 
 int b200q_launch_dequant_bf16_experts(const void * W, const b200q_layout & L, void * out, int e0, int n_e, const int * bounds, cudaStream_t st);
 int b200q_launch_wire_dequant_bf16_experts(int type, const void * W, int64_t M, int64_t K, int64_t estride, void * out, int e0, int n_e, const int * bounds, cudaStream_t st);
 int b200q_moe_gemm_shape_ok(int type, int64_t M, int64_t K, int n_used, int nb1, int n_tokens, int n_expert, int up_gate);
-size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate);
+size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate, int64_t rows_layout);
 int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_bytes, cudaStream_t st);
+
+// row origins of the MoE operands (b200q_mmvq_id_desc, b200q_moe_gemm), resolved on the host: bytes from the start of plane p to row `row0`
+// (wire-layout types: of the verbatim tensor, row0 a multiple of the row interleave); rows [row0, ...) of a tensor then read like a tensor of
+// their own, with the plane offsets of the whole one
+static inline int64_t b200q_row_offset(const b200q_layout & L, int p, int64_t row0) {
+    if (L.wire) return p == 0 ? row0 * ((int64_t)L.row_meta + L.nb * L.wire_block) : 0;
+    return row0 * (L.plane_per_row[p] ? 1 : L.nb) * L.plane_bytes[p];
+}
+static inline b200q_planes b200q_planes_at(const uint8_t * base, const b200q_layout & L, int64_t row0) {
+    b200q_planes P = b200q_planes_from(base, L);
+    for (int i = 0; i < B200Q_MAX_PLANES; ++i) P.p[i] += b200q_row_offset(L, i, row0);
+    return P;
+}

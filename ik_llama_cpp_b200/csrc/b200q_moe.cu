@@ -9,7 +9,8 @@
 //   2. k_f32_to_bf16 with a row map: the bf16 B operand [slot][K] in sorted order.
 //   3. the grouped GEMM (b200q_launch_gemm_grouped): k_gemm_q<.., GROUPED> for the fused types, dequantise-the-active-experts + k_gemm_bf16<.., GROUPED>
 //      for the others; the epilogue stores each column straight to dst[slot].
-//   4. up/gate: up and gate are two segments of that launch (up -> workspace, gate -> dst), then k_mul_unary over n_slots x M.
+//   4. up/gate: up and gate are two segments of that launch (up -> workspace, gate -> dst), then k_mul_unary over n_slots x M.  Merged up/gate
+//      experts ([gate; up] in one [2 M x K] matrix per expert) are the same two segments over row ranges of one tensor (b200q_moe_gemm::row0).
 // The reference's generic path (ggml_cuda_mul_mat_id, ggml-cuda.cu:2836-2950) copies ids to the host and synchronises to build its row mapping.
 #include "b200q_internal.h"
 #include <cuda_runtime.h>
@@ -68,7 +69,8 @@ k_moe_route(const int32_t * __restrict__ ids, int n_slots, int n_used, int nb1, 
 int moe_tile_rows(int64_t n_slots, int n_expert) { return n_slots >= (int64_t)256 * n_expert ? 256 : 128; }
 
 struct moe_ws_layout { size_t bounds, tile_start, tiles, slot, col, xb, up, wsc, wsc_bytes, total; };
-moe_ws_layout moe_layout(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate) {
+// rows_layout: rows of one expert matrix (M, or 2 M for merged up/gate experts, whose generic-type scratch holds both halves)
+moe_ws_layout moe_layout(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate, int64_t rows_layout) {
     moe_ws_layout L; size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off += (size_t)b200q_align_up((int64_t)bytes, 256); return o; };
     const int64_t max_tiles = (n_slots + 127) / 128 + std::min<int64_t>(n_expert, n_slots);
@@ -76,7 +78,7 @@ moe_ws_layout moe_layout(int type, int64_t M, int64_t K, int64_t n_slots, int n_
     L.slot = take(sizeof(int) * n_slots); L.col = take(sizeof(int) * n_slots);
     L.xb = take((size_t)n_slots * K * 2);
     L.up = up_gate ? take((size_t)n_slots * M * 4) : 0;
-    const int64_t ebytes = M * K * 2;
+    const int64_t ebytes = rows_layout * K * 2;
     L.wsc_bytes = b200q_gemm_fused_type(type) ? 0 : (size_t)(std::min<int64_t>(n_expert, std::max<int64_t>(1, MOE_SCRATCH_BUDGET / ebytes)) * ebytes);
     L.wsc = take(L.wsc_bytes);
     L.total = off;
@@ -94,8 +96,8 @@ int b200q_moe_gemm_shape_ok(int type, int64_t M, int64_t K, int n_used, int nb1,
     b200q_layout L; return b200q_make_layout(type, M, K, &L) == 0 ? 1 : 0;
 }
 
-size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate) {
-    return moe_layout(type, M, K, n_slots, n_expert, up_gate).total;
+size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate, int64_t rows_layout) {
+    return moe_layout(type, M, K, n_slots, n_expert, up_gate, rows_layout).total;
 }
 
 int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_bytes, cudaStream_t st) {
@@ -103,7 +105,7 @@ int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_byt
     if (!b200q_moe_gemm_shape_ok(d.type, d.M, d.K, d.n_used, d.nb1, d.n_tokens, d.n_expert, ug)) return -2;
     if (((uintptr_t)d.x & 15) || ((uintptr_t)ws & 255)) return -2;
     const int64_t n_slots = (int64_t)d.n_tokens * d.n_used;
-    const moe_ws_layout L = moe_layout(d.type, d.M, d.K, n_slots, d.n_expert, ug);
+    const moe_ws_layout L = moe_layout(d.type, d.M, d.K, n_slots, d.n_expert, ug, d.rows_layout);
     if (ws_bytes < L.total) return -5;
     char * b = (char *)ws;
     int * bounds = (int *)(b + L.bounds), * tile_start = (int *)(b + L.tile_start), * slot = (int *)(b + L.slot), * col = (int *)(b + L.col);
@@ -115,6 +117,7 @@ int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_byt
     if ((rc = b200q_launch_f32_to_bf16_rows(d.x, col, b + L.xb, d.K, n_slots, st))) return rc;
     b200q_moe_gemm g{};
     g.type = d.type; g.n_seg = ug ? 2 : 1; g.W[0] = d.W; g.dst[0] = ug ? up : d.dst; g.W[1] = d.W2; g.dst[1] = d.dst;
+    g.row0[0] = d.W_row0; g.row0[1] = d.W2_row0; g.rows_layout = d.rows_layout;
     g.M = d.M; g.K = d.K; g.n_expert = d.n_expert; g.n_rows = n_slots; g.xb = b + L.xb; g.bn = bn;
     g.rt = b200q_moe_route{bounds, tile_start, tiles, slot, 0, d.n_expert};
     if ((rc = b200q_launch_gemm_grouped(g, b + L.wsc, L.wsc_bytes, st))) return rc;

@@ -202,9 +202,11 @@ int launch_wire_mmvq_id_t(const wire_id_args & a, bool upgate, int sm_count, boo
 
 int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
     const int rc = b200q_wire_check(d.type, d.M, d.K); if (rc) return rc;
-    b200q_layout L; if (b200q_make_layout(d.type, d.M, d.K, &L)) return -1;
+    b200q_layout L; if (const int lr = b200q_make_layout(d.type, d.rows_layout, d.K, &L)) return lr;
+    if (d.W_row0 % L.wire || d.W2_row0 % L.wire) return -2;          // a row origin inside a group of interleaved rows
     wire_id_args a; memset(&a, 0, sizeof a);
-    a.W = (const uint8_t *)d.W; a.W2 = (const uint8_t *)d.W2; a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used;
+    a.W = (const uint8_t *)d.W + b200q_row_offset(L, 0, d.W_row0); a.W2 = d.W2 ? (const uint8_t *)d.W2 + b200q_row_offset(L, 0, d.W2_row0) : nullptr;
+    a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used;
     a.n_used = d.n_used; a.nb1 = d.nb1; a.ncx = d.n_tokens * d.nb1; a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit;
     switch (d.type) {
 #define X(T) case T: return launch_wire_mmvq_id_t<T>(a, d.W2 != nullptr, d.sm_count, d.pdl != 0, st);

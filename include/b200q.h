@@ -177,6 +177,18 @@ B200Q_API int b200q_mul_mat_id_gemm(int type, const void * W, const void * W_gat
                           int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
 B200Q_API int b200q_mul_mat_id(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
                      int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
+/* ---- MoE with merged up/gate experts: GGML_OP_MOE_FUSED_UP_GATE with src[0] = ffn_gate_up_exps [k, 2 m, n_expert], src[1] = NULL, no biases ----
+ * (ggml_moe_up_gate(ctx, up_gate_exps, NULL, ...), the reference CPU op iqk_moe_fused_up_gate: ggml.c:18620-18632).  W_gate_up: n_expert matrices
+ * [2 m x k] of `type` in the device layout, b200q_plane_bytes(type, 2 m, k) apart (each uploaded whole with b200q_set_tensor); rows [0, m) of a matrix
+ * are the GATE rows, rows [m, 2 m) the UP rows:  dst[t][e][i] = unary(gate_i(id) . x) * (up_i(id) . x), id = ids[t][e], with the unary / limit rules
+ * and the ids, x, dst conventions of b200q_mul_mat_id (ids outside [0, n_expert) give zero rows).  Shape conditions: k a multiple of the type's block
+ * (of 256 for the grouped GEMM, else the mat-vec serves every batch); for the types whose rows are interleaved in groups of 4 (_R4), m % 4 == 0.
+ * Same arithmetic, launches and crossover as b200q_mul_mat_id on the two halves uploaded as separate tensors.
+ * b200q_moe_up_gate_merged_workspace: bytes of device workspace, 0 exactly when b200q_moe_up_gate_merged takes the mat-vec path (then workspace may
+ * be NULL); needs no device.  b200q_moe_up_gate_merged: the dispatcher; no host round trip, allocation or synchronisation (capturable). */
+B200Q_API size_t b200q_moe_up_gate_merged_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert);
+B200Q_API int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_expert, const int32_t * ids, const float * x, float * dst,
+                             int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
 /* same through HOST activations/results: H2D(x) -> mul_mat -> D2H(dst), synchronous (end-to-end entry point) */
 B200Q_API int b200q_mul_mat_host(int type, const void * W_planes_dev, const float * x_host, float * dst_host,
                        int64_t m, int64_t k, int64_t n, void * stream);

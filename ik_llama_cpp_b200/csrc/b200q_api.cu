@@ -317,7 +317,8 @@ size_t b200q_mul_mat_multi_workspace(int type, int n_tensors, const int64_t * m,
 int b200q_mul_mat_multi(int type, int n_tensors, const void * const * W, float * const * dst, const int64_t * m, int64_t k,
                         const float * x, int64_t n, void * workspace, size_t workspace_bytes, void * stream) {
     if (n <= 8) return b200q_mul_mat_vec_multi(type, n_tensors, W, dst, m, k, x, (int)n, k, stream);
-    if (!x || !workspace || workspace_bytes < b200q_mul_mat_multi_workspace(type, n_tensors, m, k, n)) return fail(B200Q_E_ARG, "b200q_mul_mat_multi: bad argument / workspace too small");
+    if (!x || !workspace) return fail(B200Q_E_ARG, "b200q_mul_mat_multi: bad argument");
+    if (workspace_bytes < b200q_mul_mat_multi_workspace(type, n_tensors, m, k, n)) return fail(B200Q_E_NOMEM, "b200q_mul_mat_multi: workspace too small");
     int rc = b200q_convert_f32_bf16(x, k, workspace, k, n, stream); if (rc) return rc;
     const size_t off = (size_t)b200q_align_up(n * k * 2, 256);
     return b200q_mul_mat_gemm_multi_bf16(type, n_tensors, W, dst, m, k, workspace, n, (char *)workspace + off, workspace_bytes - off, stream);
@@ -334,7 +335,7 @@ int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_ga
     if (!W_up || !W_gate || !x_bf16 || !dst || !workspace || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_fused_up_gate_gemm_bf16: bad argument");
     dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_fused_up_gate_gemm_bf16: no CUDA device");
     const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
-    if (workspace_bytes < up_bytes) return fail(B200Q_E_ARG, "b200q_fused_up_gate_gemm_bf16: workspace too small");
+    if (workspace_bytes < up_bytes) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate_gemm_bf16: workspace too small");
     float * up_res = (float *)workspace; void * wsc = (char *)workspace + up_bytes; const size_t wsc_bytes = workspace_bytes - up_bytes;
     cudaStream_t st = (cudaStream_t)stream;
     // up and gate as the two segments of ONE launch (up -> workspace, gate -> dst), then the unary-mul tail in place, which also writes dst_bf16
@@ -347,7 +348,8 @@ int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_ga
 int b200q_fused_up_gate(int type, const void * W_up, const void * W_gate, const float * x, float * dst, int64_t m, int64_t k, int64_t n,
                         int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
     if (n <= 8) return b200q_fused_up_gate_vec(type, W_up, W_gate, x, dst, m, k, (int)n, k, unary, limit, stream);
-    if (!x || !workspace || workspace_bytes < b200q_fused_up_gate_workspace(type, m, k, n)) return fail(B200Q_E_ARG, "b200q_fused_up_gate: bad argument / workspace too small");
+    if (!x || !workspace) return fail(B200Q_E_ARG, "b200q_fused_up_gate: bad argument");
+    if (workspace_bytes < b200q_fused_up_gate_workspace(type, m, k, n)) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate: workspace too small");
     if ((m * n) % 4) return fail(B200Q_E_SHAPE, "b200q_fused_up_gate: m*n must be a multiple of 4");
     int rc;
     {   // ternary weights: both GEMMs on the int8 tensor pipe (one activation quantisation, one launch over the up and gate row tiles), then the unary-mul tail

@@ -806,8 +806,9 @@ int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t
     return d.N > 128 ? launch_gemm_bn_i8<1>(d, xq, ts, sx, st) : launch_gemm_bn_i8<0>(d, xq, ts, sx, st);
 }
 
-// dst[j][i] = a[j][i] + b[j % nb][i]  (GGML_OP_ADD of a mat-mul result with a bias row / a same-shape tensor, when it is NOT fused into the mat-vec)
-__global__ void k_add_rows(const float * __restrict__ a, const float * __restrict__ b, float * __restrict__ dst, int64_t m, int64_t n, int64_t nb) {
+// dst[j][i] = a[j][i] + b[j % nb][i]  (GGML_OP_ADD of a mat-mul result with a bias row / a same-shape tensor, when it is NOT fused into the mat-vec).
+// dst may be a or b (an in-place ADD of ggml's allocator): no __restrict__ on the operands
+__global__ void k_add_rows(const float * a, const float * b, float * dst, int64_t m, int64_t n, int64_t nb) {
     const int64_t total = m * n;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) dst[i] = a[i] + b[((i / m) % nb) * m + i % m];
 }
@@ -863,10 +864,15 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         if (k_split > 1) for (int i = 0; i < d.n_seg; ++i) { cudaError_t e = cudaMemsetAsync(d.dst[i], 0, (size_t)d.M[i] * N * sizeof(float), st); if (e != cudaSuccess) return -3; }
         return launch_gemm_q<false>(type, bn256, d, k_split, 1, b200q_moe_route{}, nullptr, st);
     }
-    // unfused: bf16 weight scratch + plain bf16 GEMM per tensor; tile / split selection: fill ~1 wave of the SMs
+    // unfused: bf16 weight scratch + plain bf16 GEMM per tensor; tile / split selection: fill ~1 wave of the SMs.
+    // Every segment's type and scratch size is checked before the first memset or launch: an error return leaves every dst untouched.
+    for (int i = 0; i < d.n_seg; ++i) {
+        b200q_layout L; if (b200q_make_layout(type, d.M[i], K, &L)) return -1;
+        if (ws_bytes < (size_t)b200q_align_up(d.M[i] * K * 2, 256)) return -5;
+    }
     for (int i = 0; i < d.n_seg; ++i) {
         const int64_t M = d.M[i];
-        b200q_layout L; if (b200q_make_layout(type, M, K, &L)) return -1;
+        b200q_layout L; b200q_make_layout(type, M, K, &L);
         const int64_t mt = (M + BM - 1) / BM;
         const bool bn256 = N >= 256 && mt * ((N + 255) / 256) >= sm_count / 2;
         const int64_t tiles = bn256 ? mt * ((N + 255) / 256) : mt * ((N + 127) / 128);
@@ -874,7 +880,6 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         const int64_t nk = (K + BK - 1) / BK;
         while (tiles * k_split * 2 <= sm_count && k_split * 2 <= 8 && nk / (k_split * 2) >= 8) k_split *= 2;
         if (k_split > 1) { cudaError_t e = cudaMemsetAsync(d.dst[i], 0, (size_t)M * N * sizeof(float), st); if (e != cudaSuccess) return -3; }
-        if (ws_bytes < (size_t)b200q_align_up(M * K * 2, 256)) return -5;
         int rc = b200q_launch_dequant_bf16(d.W[i], L, wscratch, st); if (rc) return rc;
         rc = bn256 ? launch_gemm_bf16<256, false>(wscratch, 1, M, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st)
                    : launch_gemm_bf16<128, false>(wscratch, 1, M, d.xb, d.dst[i], M, N, K, k_split, b200q_moe_route{}, st);

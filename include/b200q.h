@@ -18,6 +18,14 @@
  *   b200q_reduce_*                         ggml_cuda_op_reduce                                 ggml-cuda/reduce.cu:125-598
  * Tensor conventions are ggml's: W is [M rows][K cols] in the GGUF wire format of `type`
  * (row stride = ggml_row_size(type, K)); x is f32 [N][K]; dst is f32 [N][M]  (dst[j*M + i]).
+ *
+ * Memory contract of every compute entry point (tests/test_gpu_memory_contract.py checks it on guarded buffers):
+ *   - a call writes only its dst(s), its extra outputs (dst_bf16, the q8 image), and at most the queried or documented workspace bytes;
+ *   - W, x, x_bf16, ids, bias and a q8 image passed as input are read-only;
+ *   - the result does not depend on what the outputs or the workspace held before the call: every output element is written (never
+ *     accumulated into), and one workspace may be reused across calls of any shape;
+ *   - an argument, type, shape or workspace error returns before anything is written.  A workspace smaller than the query or the
+ *     documented size returns B200Q_E_NOMEM.
  */
 #ifndef B200Q_H
 #define B200Q_H
@@ -98,7 +106,7 @@ B200Q_API int b200q_mul_mat_gemm_multi_bf16(int type, int n_tensors, const void 
 /* GGML_OP_FUSED_UP_GATE for n > 8 (ggml_cuda_up_gate_unary, ggml-cuda.cu:3588-3618: two MMQ + ggml_fused_mul_unary): up and gate
  * are the two segments of one GEMM launch, followed by one elementwise unary-mul pass; dst_bf16 (optional, may be NULL) receives a
  * bf16 copy = the operand of ffn_down.
- * workspace >= align256(m*n*4) + align256(m*k*2) */
+ * workspace >= align256(m*n*4) (the up result) + align256(m*k*2) (the bf16 weight scratch, only for types without a fused kernel) */
 B200Q_API int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_gate, const void * x_bf16, float * dst, void * dst_bf16,
                                   int64_t m, int64_t k, int64_t n, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
 

@@ -1,6 +1,7 @@
 // b200q_api.cu — the C ABI of libb200q.so (see include/b200q.h for the reference interfaces each entry replaces).
 #include "../../include/b200q.h"
 #include "b200q_internal.h"
+#include "b200q_decode_plan.h"
 #include <cuda_runtime.h>
 #include <mutex>
 #include <stdarg.h>
@@ -147,11 +148,11 @@ static int mmvq_cols(b200q_mmvq_desc & d, int n, int64_t x_stride, cudaStream_t 
     if (((uintptr_t)d.x & 15) || (xs & 3)) return fail(B200Q_E_ARG, "%s: activations must be 16-byte aligned with a row stride multiple of 4 floats", what);
     float * dst0[B200Q_MAX_SEGS]; for (int i = 0; i < d.n_seg; ++i) dst0[i] = d.seg[i].dst;
     const float * x0 = d.x;
+    const int64_t max_cols = b200q_mmvq_max_cols(d.K);
     while (done < n) {
         int c = 8; while (c > n - done) c >>= 1;
-        // shared memory budget: c*K int8 + c*(K/32)*8 bytes must fit in ~200 KB
-        while (c > 1 && (size_t)c * d.K + (size_t)c * (d.K / 32) * 8 > 200 * 1024) c >>= 1;
-        if ((size_t)c * d.K + (size_t)c * (d.K / 32) * 8 > 200 * 1024) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)d.K);
+        while (c > 1 && c > max_cols) c >>= 1;
+        if (c > max_cols) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)d.K);
         d.ncols = c; d.x = x0 + (int64_t)done * xs; d.x_stride = xs;
         for (int i = 0; i < d.n_seg; ++i) d.seg[i].dst = dst0[i] + (int64_t)done * d.seg[i].M;
         int rc = check_launch(b200q_launch_mmvq(d, st), what);
@@ -206,14 +207,11 @@ int b200q_fused_up_gate_vec_q8(int type, const void * W_up, const void * W_gate,
     d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
     if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_fused_up_gate_vec_q8: activations must be 16-byte aligned");
     attach_next(d);
-    if (q8_out && opt_q8()) {
-        d.q8_out = q8_out;
-        const int rc = b200q_launch_mmvq(d, (cudaStream_t)stream);
-        if (rc == 0) { if (q8_produced) *q8_produced = 1; return B200Q_OK; }
-        if (rc != -8) return check_launch(rc, "b200q_fused_up_gate_vec_q8");
-        d.q8_out = nullptr;              // shape not eligible for the hand-off: plain launch
-    }
-    return check_launch(b200q_launch_mmvq(d, (cudaStream_t)stream), "b200q_fused_up_gate_vec_q8");
+    if (q8_out && opt_q8()) d.q8_out = q8_out;     // a shape not eligible for the hand-off is planned as the plain launch
+    b200q_mmvq_plan p;
+    const int rc = check_launch(b200q_launch_mmvq(d, (cudaStream_t)stream, &p), "b200q_fused_up_gate_vec_q8");
+    if (rc == 0 && q8_produced) *q8_produced = p.q8 == 2;
+    return rc;
 }
 int b200q_mul_mat_vec_q8(int type, const void * W, const float * x, const void * q8_in, float * dst, int64_t m, int64_t k,
                          const float * bias, void * stream) {
@@ -223,13 +221,7 @@ int b200q_mul_mat_vec_q8(int type, const void * W, const float * x, const void *
     d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst, bias, m}; d.K = k; d.x = x; d.x_stride = k; d.ncols = 1; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
     if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_q8: activations must be 16-byte aligned");
     attach_next(d);
-    if (q8_in && opt_q8()) {
-        d.q8_in = q8_in;
-        const int rc = b200q_launch_mmvq(d, (cudaStream_t)stream);
-        if (rc == 0) return B200Q_OK;
-        if (rc != -8) return check_launch(rc, "b200q_mul_mat_vec_q8");
-        d.q8_in = nullptr;
-    }
+    if (q8_in && opt_q8()) d.q8_in = q8_in;
     return check_launch(b200q_launch_mmvq(d, (cudaStream_t)stream), "b200q_mul_mat_vec_q8");
 }
 
@@ -351,20 +343,17 @@ int b200q_fused_up_gate(int type, const void * W_up, const void * W_gate, const 
     if (!x || !workspace) return fail(B200Q_E_ARG, "b200q_fused_up_gate: bad argument");
     if (workspace_bytes < b200q_fused_up_gate_workspace(type, m, k, n)) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate: workspace too small");
     if ((m * n) % 4) return fail(B200Q_E_SHAPE, "b200q_fused_up_gate: m*n must be a multiple of 4");
-    int rc;
-    {   // ternary weights: both GEMMs on the int8 tensor pipe (one activation quantisation, one launch over the up and gate row tiles), then the unary-mul tail
-        dev_info & di = device_info();
-        const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
-        if (type == B200Q_TYPE_IQ2_BN && opt_fused() && di.ok && workspace_bytes >= up_bytes + b200q_gemm_i8_workspace_bytes(k, n)) {
-            float * up_res = (float *)workspace;
-            b200q_gemm_multi d; memset(&d, 0, sizeof d);
-            d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n;
-            rc = b200q_launch_gemm_bn_i8(d, x, k, (char *)workspace + up_bytes, workspace_bytes - up_bytes, (cudaStream_t)stream);
-            if (rc == 0) return check_launch(b200q_launch_mul_unary(dst, up_res, dst, nullptr, m * n, unary, limit, (cudaStream_t)stream), "b200q_fused_up_gate(unary)");
-            if (rc != -100) return check_launch(rc, "b200q_fused_up_gate(int8)");
-        }
+    // ternary weights: both GEMMs on the int8 tensor pipe (one activation quantisation, one launch over the up and gate row tiles), then the unary-mul tail
+    const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
+    if (opt_fused() && device_info().ok && b200q_gemm_bn_i8_ok(type, k, n, x, k, workspace_bytes - up_bytes)) {
+        float * up_res = (float *)workspace;
+        b200q_gemm_multi d; memset(&d, 0, sizeof d);
+        d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n;
+        const int rc = check_launch(b200q_launch_gemm_bn_i8(d, x, k, (char *)workspace + up_bytes, workspace_bytes - up_bytes, (cudaStream_t)stream), "b200q_fused_up_gate(int8)");
+        if (rc) return rc;
+        return check_launch(b200q_launch_mul_unary(dst, up_res, dst, nullptr, m * n, unary, limit, (cudaStream_t)stream), "b200q_fused_up_gate(unary)");
     }
-    rc = b200q_convert_f32_bf16(x, k, workspace, k, n, stream); if (rc) return rc;
+    int rc = b200q_convert_f32_bf16(x, k, workspace, k, n, stream); if (rc) return rc;
     const size_t off = (size_t)b200q_align_up(n * k * 2, 256);
     return b200q_fused_up_gate_gemm_bf16(type, W_up, W_gate, workspace, dst, nullptr, m, k, n, unary, limit, (char *)workspace + off, workspace_bytes - off, stream);
 }
@@ -396,8 +385,7 @@ static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t
     if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
     // the quantised activation columns of a launch live in shared memory: larger batches are walked in token chunks (same kernel, the expert ids
     // never leave the device).  Prefill batches are served by the grouped GEMM (b200q_mul_mat_id_gemm) once b200q_mul_mat_id selects it.
-    const int64_t col_bytes = (int64_t)nb1 * (k + k / 4);
-    int chunk = (int)((200 * 1024) / (col_bytes > 0 ? col_bytes : 1));
+    int chunk = (int)(b200q_mmvq_max_cols(k) / nb1);
     static const int forced = [] { const char * e = getenv("B200Q_MOE_CHUNK_TOKENS"); return e ? atoi(e) : 0; }();
     if (forced > 0 && forced < chunk) chunk = forced;
     if (chunk < 1) return fail(B200Q_E_SHAPE, "%s: one token's activation columns do not fit shared memory", what);

@@ -1,10 +1,11 @@
-// b200q_decode_ring.cuh — the decode mat-vec kernels (k_mmvq, k_mmvq_ring) and their per-type launcher template.
-// Included by b200q_decode.cu (dispatcher; declares the per-type launchers extern) and by the b200q_decode_i<N>.cu instantiation units,
+// b200q_decode_ring.cuh — the decode mat-vec kernels (k_mmvq, k_mmvq_ring, k_mmvq_id) and, per type, the kernel each launch plan selects.
+// Included by b200q_decode.cu (planner and launcher; declares the per-type selections extern) and by the b200q_decode_i<N>.cu instantiation units,
 // which split the 23 x 17 kernel instantiations over several translation units so that they compile in parallel.
 #pragma once
 #include "b200q_types.cuh"
 #include "b200q_internal.h"
 #include "b200q_decode_common.cuh"
+#include "b200q_decode_plan.h"
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -242,26 +243,7 @@ __global__ void __launch_bounds__(512, 1) k_mmvq_id(const mmvq_id_args a) {
     }
 }
 template <int TYPE>
-int launch_mmvq_id_type(const mmvq_id_args & a, bool upgate, int sm_count, bool pdl, cudaStream_t st) {
-    const size_t smem = (size_t)a.ncx * a.K + (size_t)a.ncx * (a.K / 32) * 8;
-    if (smem > 200 * 1024) return -2;
-    static size_t configured[2][B200Q_MAX_DEVICES] = {};
-    const int dev = b200q_current_device();
-    if (smem > 48 * 1024 && smem > configured[upgate][dev]) {
-        const cudaError_t e = upgate ? cudaFuncSetAttribute(k_mmvq_id<TYPE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                     : cudaFuncSetAttribute(k_mmvq_id<TYPE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return -3;
-        configured[upgate][dev] = smem;
-    }
-    const int nwarps = 16;
-    int64_t grid = ((int64_t)a.n_slots * a.M + nwarps - 1) / nwarps; if (grid > sm_count) grid = sm_count; if (grid < 1) grid = 1;
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(nwarps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    return upgate ? (int)cudaLaunchKernelEx(&cfg, k_mmvq_id<TYPE, true>, a) : (int)cudaLaunchKernelEx(&cfg, k_mmvq_id<TYPE, false>, a);
-}
+const void * mmvq_id_kernel(bool upgate) { return upgate ? (const void *)k_mmvq_id<TYPE, true> : (const void *)k_mmvq_id<TYPE, false>; }
 
 // ------------------------------------------------------------------------------------------------
 // decode mat-vec, TMA-ring variant (the default): weights are streamed HBM -> shared memory by cp.async.bulk (1-D TMA)
@@ -302,18 +284,6 @@ int launch_mmvq_id_type(const mmvq_id_args & a, bool upgate, int sm_count, bool 
 #define B200Q_SMEM_BUDGET (112 * 1024)   // dynamic shared memory per CTA: two CTAs per SM (same kernel, or this one + the next under PDL)
 #endif
 #define B200Q_PAIR_SLOTS 124         // ncw * S stage descriptors (+ the claim counter) fit the 128-int slot table
-struct ring_geom {
-    int n_planes;                 // block planes staged through the ring (the per-row scale plane is read directly)
-    int b8[4];                    // bytes per 8 items (256 weights) of plane p
-    int seg_off[4];               // byte offset of plane p inside a stage
-    int stage_bytes;              // 16-byte aligned
-    int n_stages;                 // S
-    int row_plane;                // index of the per-row plane in b200q_planes::p, or -1
-    int merged;                   // 1: the row is ONE segment, so the two rows of a pair are adjacent inside every plane and travel as one bulk copy per
-                                  //    plane (half as many copies in flight: tools/membench.cu `r` shows the bandwidth falling with the copy count);
-                                  //    the stage is then laid out plane-major [p0 row0 | p0 row1 | p1 row0 | p1 row1 ...]
-    int row1[4];                  // byte offset of row 1 of the pair relative to row 0, per plane
-};
 struct mmvq_ring_args {
     mmvq_args  a;
     ring_geom  g;
@@ -735,205 +705,25 @@ __global__ void __launch_bounds__(32 * (B200Q_RING_CONSUMERS + 1), B200Q_MIN_CTA
 #endif
 }
 
-template <int TYPE, int NCOLS, bool UPGATE>
-static int launch_mmvq_t(const mmvq_args & a, int sm_count, bool pdl, cudaStream_t st) {
-    const size_t smem = (size_t)NCOLS * a.K + (size_t)NCOLS * (a.K / 32) * 8;
-    static size_t configured[B200Q_MAX_DEVICES] = {};     // function attributes are per device
-    const int dev = b200q_current_device();
-    if (smem > 48 * 1024 && smem > configured[dev]) {
-        if (cudaFuncSetAttribute(k_mmvq<TYPE, NCOLS, UPGATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -3;
-        configured[dev] = smem;
-    }
-    // one warp per row, one CTA per SM; shrink the CTA when there are fewer rows than warps
-    int nwarps = 16;
-    while (nwarps > 2 && a.M_total <= (int64_t)sm_count * (nwarps / 2)) nwarps >>= 1;
-    int64_t grid = (a.M_total + nwarps - 1) / nwarps;
-    if (grid > sm_count) grid = sm_count;
-    if (grid < 1) grid = 1;
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(nwarps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    return (int)cudaLaunchKernelEx(&cfg, k_mmvq<TYPE, NCOLS, UPGATE>, a);
-}
-
-// ring geometry for a type; returns false if the planes cannot be bulk-copied (alignment) -> LDG kernel
-// long_rows: K > 4096: a stage holds up to 2 x B200Q_SEG_ITEMS items of ONE row (plane-major), else a pair of single-segment rows
-static bool make_ring_geom(int type, int64_t K, ring_geom & g, bool long_rows) {
-    b200q_layout L; if (b200q_make_layout(type, 1, K, &L)) return false;
-    if (K % 32) return false;
-    // K % 256 != 0 (32- / 64-weight block types only: bitnet's IQ2_BN rows of 3200 / 8640): fine as long as every plane row is a whole number of
-    // bytes and stays 16-byte aligned (checked per plane below)
-    const int64_t n32 = K / 32;
-    memset(&g, 0, sizeof g); g.row_plane = -1;
-    int off = 0, np = 0;
-    for (int p = 0; p < L.n_planes; ++p) {
-        if (L.plane_per_row[p]) { g.row_plane = p; continue; }
-        if (p != np) return false;                       // block planes must come first (they do for every type)
-        const int b8 = L.plane_bytes[p] * 256 / L.qk;
-        if (b8 <= 0 || (n32 * b8) % 128) return false;   // every row/segment start must be 16-byte aligned: row bytes = n32 * b8 / 8
-        g.b8[np] = b8; g.seg_off[np] = off; off += (int)b200q_align_up((B200Q_SEG_ITEMS / 8) * b8, 16); ++np;
-    }
-    g.n_planes = np; g.stage_bytes = (int)b200q_align_up(off, 128);
-    for (int p = 0; p < np; ++p) g.row1[p] = g.stage_bytes;          // row-major stage: [row 0: planes][row 1: planes]
-    // one segment per row: merge the two rows of a pair into one copy per plane (B200Q_MERGE_PAIR=0 restores the round-1 scheme)
-    static const int merge = [] { const char * e = getenv("B200Q_MERGE_PAIR"); return e ? atoi(e) : 1; }();
-    if (long_rows) {
-        int o = 0;
-        for (int p = 0; p < np; ++p) { const int hb = (B200Q_SEG_ITEMS / 8) * g.b8[p]; g.seg_off[p] = o; g.row1[p] = hb; o += (int)b200q_align_up(2 * hb, 16); }
-        g.merged = 1;
-    } else if (merge && K / 32 <= B200Q_SEG_ITEMS && np > 0 && np <= 4) {
-        int o = 0;
-        for (int p = 0; p < np; ++p) { const int rb = (int)((n32 * g.b8[p]) >> 3); g.seg_off[p] = o; g.row1[p] = rb; o += (int)b200q_align_up(2 * rb, 16); }
-        if (o <= 2 * g.stage_bytes) g.merged = 1;
-        else { int o2 = 0; for (int p = 0; p < np; ++p) { g.seg_off[p] = o2; o2 += (int)b200q_align_up((B200Q_SEG_ITEMS / 8) * g.b8[p], 16); g.row1[p] = g.stage_bytes; } }
-    }
-    return np > 0 && np <= 4;
-}
-
-// consumer warps / stages of a ring launch (shared by the launcher and by the L2 warm-up of the next launch)
-static inline size_t ring_xbytes(int ncols, int64_t K) { return (size_t)ncols * K + (size_t)ncols * (K / 32) * 8 + 512 + 512 + 256 + 128; }
-static inline bool ring_shape(int ncols, int64_t K, size_t pair_stage, int64_t n_units, int sm_count, int & ncw, int & S) {
-    const size_t xbytes = ring_xbytes(ncols, K), budget = B200Q_SMEM_BUDGET;
-    ncw = B200Q_RING_CONSUMERS; S = 0;                   // consumer warps (+1 producer warp)
-    for (;;) {
-        const size_t per_stage = (size_t)ncw * (pair_stage + 16);
-        S = xbytes + 64 < budget ? (int)((budget - xbytes - 64) / per_stage) : 0;
-        if (S >= 2 || ncw == 3) break;
-        ncw = ncw > 19 ? 19 : ncw > 15 ? 15 : ncw > 11 ? 11 : ncw > 7 ? 7 : 3;      // (10 warps would still fit two stages for K = 14336 but measured slower: 13.8 vs 11.3 us)
-    }
-    if (S < 2) return false;
-    if (S > B200Q_MAX_STAGES) S = B200Q_MAX_STAGES;
-    while (ncw > 3 && n_units <= (int64_t)sm_count * (ncw > 7 ? 7 : 3)) ncw = ncw > 7 ? 7 : 3;
-    while (ncw * S > B200Q_PAIR_SLOTS) --S;
-    return true;
-}
-// what the next decode launch (descriptor nx) will request first -> mmvq_pf (see struct mmvq_pf)
-static inline void make_next_prefetch(const b200q_mmvq_desc & nx, int sm_count, int ctas_per_sm, mmvq_pf & pf) {
-    memset(&pf, 0, sizeof pf);
-    if (nx.n_seg < 1 || nx.ncols > 2 || nx.tp.in || nx.tp.out) return;
-    const bool upgate = nx.seg[0].W2 != nullptr;
-    int64_t M_total = 0; for (int i = 0; i < nx.n_seg; ++i) M_total += nx.seg[i].M;
-    if (b200q_is_wire_type(nx.type)) {                   // wire-layout tensors: whole (or the head of) each tensor
-        b200q_layout L;
-        for (int i = 0; i < nx.n_seg && pf.n < 8; ++i) for (int t = 0; t < (upgate ? 2 : 1) && pf.n < 8; ++t) {
-            if (b200q_make_layout(nx.type, nx.seg[i].M, nx.K, &L)) return;
-            pf.ptr[pf.n] = (const uint8_t *)(t ? nx.seg[i].W2 : nx.seg[i].W); pf.bytes[pf.n] = std::min<long long>(L.M * b200q_wire_row_size(L), 24ll << 20); ++pf.n;
-        }
-        pf.mode = 0; return;
-    }
-    const bool long_rows = nx.K / 32 > B200Q_SEG_ITEMS;
-    ring_geom g;
-    if (!nx.ring || !make_ring_geom(nx.type, nx.K, g, long_rows)) return;
-    if (nx.K % 256) return;
-    const int64_t n8 = nx.K / 256;
-    const int64_t n_units = long_rows ? M_total : (M_total + 1) / 2;
-    int ncw, S; if (!ring_shape(nx.ncols, nx.K, 2 * (size_t)g.stage_bytes, n_units, sm_count, ncw, S)) return;
-    long long total = 0;
-    for (int i = 0; i < nx.n_seg; ++i) for (int p = 0; p < g.n_planes; ++p) total += (long long)nx.seg[i].M * n8 * g.b8[p] * (upgate ? 2 : 1);
-    if (nx.n_seg > 1 || total <= (24ll << 20)) {         // small: everything, split evenly over our CTAs
-        for (int i = 0; i < nx.n_seg; ++i) for (int t = 0; t < (upgate ? 2 : 1); ++t) {
-            b200q_layout L; if (b200q_make_layout(nx.type, nx.seg[i].M, nx.K, &L)) return;
-            const b200q_planes P = b200q_planes_from((const uint8_t *)(t ? nx.seg[i].W2 : nx.seg[i].W), L);
-            for (int p = 0; p < g.n_planes && pf.n < 8; ++p) { pf.ptr[pf.n] = P.p[p]; pf.bytes[pf.n] = (long long)nx.seg[i].M * n8 * g.b8[p]; ++pf.n; }
-        }
-        pf.mode = 0; return;
-    }
-    // one (or up + gate) large tensor: the first stages of every CTA of the next grid
-    const int nseg = long_rows ? (int)((nx.K / 32 + 2 * B200Q_SEG_ITEMS - 1) / (2 * B200Q_SEG_ITEMS)) : 1, nt = upgate ? 2 : 1;
-    int64_t grid = (n_units + ncw - 1) / ncw; if (grid > (int64_t)sm_count * ctas_per_sm) grid = (int64_t)sm_count * ctas_per_sm;
-    for (int t = 0; t < nt; ++t) {
-        b200q_layout L; if (b200q_make_layout(nx.type, nx.seg[0].M, nx.K, &L)) return;
-        const b200q_planes P = b200q_planes_from((const uint8_t *)(t ? nx.seg[0].W2 : nx.seg[0].W), L);
-        for (int p = 0; p < g.n_planes && pf.n < 8; ++p) { pf.ptr[pf.n] = P.p[p]; pf.rowb[pf.n] = (int)(n8 * g.b8[p]); ++pf.n; }
-    }
-    pf.mode = 1; pf.n_units = (int)n_units; pf.rpu = long_rows ? 1 : 2; pf.grid = (int)grid;
-    pf.per_cta = (ncw * S + nseg * nt - 1) / (nseg * nt);
-}
+// the kernel a plan (plan_mmvq) launches for this type.  The kernels are referenced (and so emitted) in the order of the instantiations
+// they had before, which keeps ptxas' output for them unchanged.
 template <int TYPE, int NCOLS, bool UPGATE, bool MULTI, bool PAIR, bool TP = false, int Q8 = 0>
-static int launch_mmvq_ring_tp(const mmvq_args & a, const ring_geom & g0, int sm_count, bool pdl, int ctas_per_sm, cudaStream_t st) {
-    mmvq_ring_args ra; ra.a = a; ra.g = g0;
-    if (PAIR) for (int i = 0; i < a.n_seg; ++i) if ((a.seg[i].M & 1) && i + 1 < a.n_seg) return -100;     // row pairs must not straddle tensors
-    if (a.M_total >= (int64_t)1 << 30) return -100;
-    const size_t xbytes = ring_xbytes(NCOLS, a.K);
-    const size_t budget = B200Q_SMEM_BUDGET;
-    const size_t pair_stage = 2 * (size_t)ra.g.stage_bytes;
-    const int64_t n_pairs = PAIR ? (a.M_total + 1) / 2 : a.M_total;
-    int ncw, S;
-    if (!ring_shape(NCOLS, a.K, pair_stage, n_pairs, sm_count, ncw, S)) return -100;     // does not fit: caller falls back to the LDG kernel
-    ra.g.n_stages = S;
-    size_t smem = (size_t)ncw * S * (pair_stage + 16) + xbytes + 64;
-    static bool configured[B200Q_MAX_DEVICES] = {};
-    const int dev = b200q_current_device();
-    if (!configured[dev]) {
-        if (cudaFuncSetAttribute(k_mmvq_ring<TYPE, NCOLS, UPGATE, MULTI, PAIR, TP, Q8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(budget)) != cudaSuccess) return -3;
-        configured[dev] = true;
-    }
-    // B200Q_GRID_FULL=1 (experiment): always spread over every SM, even when a CTA then has fewer units than consumer warps
-    static const int grid_full = [] { const char * e = getenv("B200Q_GRID_FULL"); return e ? atoi(e) : 0; }();
-    int64_t grid = grid_full ? n_pairs : (n_pairs + ncw - 1) / ncw;
-    if (grid > (int64_t)sm_count * ctas_per_sm) grid = (int64_t)sm_count * ctas_per_sm;
-    if (grid < 1) grid = 1;
-    if (TP && a.tp.out && !MULTI) {
-        // row buffer of a reduce_out launch: the rows of one CTA (a contiguous range, +-1 unit) are sent in one coalesced burst at the end
-        const int64_t rows = (PAIR ? 2 : 1) * ((n_pairs + grid - 1) / grid + 1) + 2;
-        // (measured at 2 GPUs: no gain, the extra CTA barrier costs more than the coalescing saves -> off by default, B200Q_TP_ROWBUF=1 enables it)
-        static const int on_env = [] { const char * e = getenv("B200Q_TP_ROWBUF"); return e ? atoi(e) : -1; }();
-        const bool on = on_env >= 0 ? on_env != 0 : a.tp.ll_peer[0] != nullptr;       // the coalescing only exists for the unicast stores
-        if (on && rows <= 2048 && smem + rows * 4 + 16 <= budget) {
-            ra.a.tp_rowbuf_off = (int)((smem + 15) & ~(size_t)15); ra.a.tp_rowbuf_rows = (int)rows;
-            smem = (size_t)ra.a.tp_rowbuf_off + rows * 4;
-        }
-    }
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((ncw + 1) * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    return (int)cudaLaunchKernelEx(&cfg, k_mmvq_ring<TYPE, NCOLS, UPGATE, MULTI, PAIR, TP, Q8>, ra);
-}
-
+static const void * ring_kernel() { return (const void *)k_mmvq_ring<TYPE, NCOLS, UPGATE, MULTI, PAIR, TP, Q8>; }
 template <int TYPE, int NCOLS, bool UPGATE, bool MULTI>
-static int launch_mmvq_ring_t(const mmvq_args & a, const ring_geom & g0, int sm_count, bool pdl, int ctas_per_sm, cudaStream_t st) {
-    // row pairs amortise the activation loads; single rows give more, shorter units when the matrix is small
-    const bool pair = a.K / 32 <= B200Q_SEG_ITEMS;         // K <= 4096: row pairs; longer rows: one row, up to 256 items per stage
-    if (a.tp.in || a.tp.out) {                             // tensor-parallel decode: n = 1
-        if (NCOLS != 1) return -7;
-        return pair ? launch_mmvq_ring_tp<TYPE, 1, UPGATE, MULTI, true, true>(a, g0, sm_count, pdl, ctas_per_sm, st)
-                    : launch_mmvq_ring_tp<TYPE, 1, UPGATE, MULTI, false, true>(a, g0, sm_count, pdl, ctas_per_sm, st);
-    }
-    if (a.q8_in || a.q8_out) {                             // q8 hand-off: n = 1, one tensor
-        if (NCOLS != 1 || MULTI) return -8;
-        if (a.q8_out) {
-            if (!UPGATE) return -8;
-            return pair ? launch_mmvq_ring_tp<TYPE, 1, true, false, true, false, 2>(a, g0, sm_count, pdl, ctas_per_sm, st)
-                        : launch_mmvq_ring_tp<TYPE, 1, true, false, false, false, 2>(a, g0, sm_count, pdl, ctas_per_sm, st);
-        }
-        if (UPGATE) return -8;
-        return pair ? launch_mmvq_ring_tp<TYPE, 1, false, false, true, false, 1>(a, g0, sm_count, pdl, ctas_per_sm, st)
-                    : launch_mmvq_ring_tp<TYPE, 1, false, false, false, false, 1>(a, g0, sm_count, pdl, ctas_per_sm, st);
-    }
-    return pair ? launch_mmvq_ring_tp<TYPE, NCOLS, UPGATE, MULTI, true>(a, g0, sm_count, pdl, ctas_per_sm, st)
-                : launch_mmvq_ring_tp<TYPE, NCOLS, UPGATE, MULTI, false>(a, g0, sm_count, pdl, ctas_per_sm, st);
+static const void * ring_kernel(const b200q_mmvq_plan & p) {
+    if (p.tp) return p.pair ? ring_kernel<TYPE, 1, UPGATE, MULTI, true, true>() : ring_kernel<TYPE, 1, UPGATE, MULTI, false, true>();
+    if (p.q8 == 2) return p.pair ? ring_kernel<TYPE, 1, true, false, true, false, 2>() : ring_kernel<TYPE, 1, true, false, false, false, 2>();
+    if (p.q8 == 1) return p.pair ? ring_kernel<TYPE, 1, false, false, true, false, 1>() : ring_kernel<TYPE, 1, false, false, false, false, 1>();
+    return p.pair ? ring_kernel<TYPE, NCOLS, UPGATE, MULTI, true>() : ring_kernel<TYPE, NCOLS, UPGATE, MULTI, false>();
 }
-
 template <int TYPE>
-int launch_mmvq_type(const mmvq_args & a, int ncols, bool upgate, int sm_count, bool pdl, bool ring, cudaStream_t st) {
-    ring_geom g;
-    if (ring && ncols <= 2 && make_ring_geom(TYPE, a.K, g, a.K / 32 > B200Q_SEG_ITEMS)) {
-        int rc;
-        static const int cps = [] { const char * e = getenv("B200Q_CTAS_PER_SM"); return e ? atoi(e) : B200Q_MIN_CTAS; }();
-        const bool multi = a.n_seg > 1;
-        if (upgate) rc = ncols == 1 ? launch_mmvq_ring_t<TYPE, 1, true, false>(a, g, sm_count, pdl, cps, st) : launch_mmvq_ring_t<TYPE, 2, true, false>(a, g, sm_count, pdl, cps, st);
-        else if (multi) rc = ncols == 1 ? launch_mmvq_ring_t<TYPE, 1, false, true>(a, g, sm_count, pdl, cps, st) : launch_mmvq_ring_t<TYPE, 2, false, true>(a, g, sm_count, pdl, cps, st);
-        else rc = ncols == 1 ? launch_mmvq_ring_t<TYPE, 1, false, false>(a, g, sm_count, pdl, cps, st) : launch_mmvq_ring_t<TYPE, 2, false, false>(a, g, sm_count, pdl, cps, st);
-        if (rc != -100) return rc;
+const void * mmvq_kernel(const b200q_mmvq_plan & p) {
+    if (p.kernel == B200Q_MMVQ_RING) {
+        if (p.upgate) return p.ncols == 1 ? ring_kernel<TYPE, 1, true, false>(p) : ring_kernel<TYPE, 2, true, false>(p);
+        if (p.multi) return p.ncols == 1 ? ring_kernel<TYPE, 1, false, true>(p) : ring_kernel<TYPE, 2, false, true>(p);
+        return p.ncols == 1 ? ring_kernel<TYPE, 1, false, false>(p) : ring_kernel<TYPE, 2, false, false>(p);
     }
-    if (a.tp.in || a.tp.out) return -7;
-    if (a.q8_in || a.q8_out) return -8;                    // only the ring kernel implements the q8 hand-off (callers retry without it)
-#define CASE(N) case N: return upgate ? launch_mmvq_t<TYPE, N, true>(a, sm_count, pdl, st) : launch_mmvq_t<TYPE, N, false>(a, sm_count, pdl, st);
-    switch (ncols) { CASE(1) CASE(2) CASE(4) CASE(8) default: return -2; }
+#define CASE(N) case N: return p.upgate ? (const void *)k_mmvq<TYPE, N, true> : (const void *)k_mmvq<TYPE, N, false>;
+    switch (p.ncols) { CASE(1) CASE(2) CASE(4) CASE(8) default: return nullptr; }
 #undef CASE
 }
-

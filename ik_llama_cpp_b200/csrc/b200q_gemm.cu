@@ -12,6 +12,7 @@
 // A comes either from the bf16 scratch written by k_dequant_bf16 (generic types) or is decoded inside the kernel (k_gemm_q, k_gemm_bn_i8).
 // With 288 threads and one CTA per SM a thread may hold up to 224 registers: the m64n256 f32 accumulator takes 128 of them.
 #include "b200q_internal.h"
+#include "b200q_decode_plan.h"
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -20,7 +21,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
-#include <unordered_map>
 
 namespace {
 
@@ -673,18 +673,6 @@ int make_tmap(CUtensorMap * tm, CUtensorMapDataType type, int rank, const void *
 }
 constexpr CUtensorMapDataType TM_BF16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, TM_U8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
 
-// opt kernel in to `bytes` of dynamic shared memory, once per device (the attribute is per device)
-int opt_in_smem(const void * kernel, size_t bytes) {
-    static std::mutex mu; static std::unordered_map<const void *, uint32_t> done;      // bit d: set on device d
-    const int dev = b200q_current_device();
-    std::lock_guard<std::mutex> lk(mu);
-    uint32_t & bits = done[kernel];
-    if (bits >> dev & 1u) return 0;
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) return -12;
-    bits |= 1u << dev;
-    return 0;
-}
-
 // activation row tiles on blockIdx.y; GROUPED: an upper bound of the tiles of n_mat experts, each expert's last tile may be partial
 template <int BN, bool GROUPED> unsigned row_tiles(int64_t N, int64_t n_mat) {
     return (unsigned)((N + BN - 1) / BN + (GROUPED ? std::min<int64_t>(n_mat, N) : 0));
@@ -699,7 +687,7 @@ int launch_gemm_bf16(const void * A_bf16, int64_t n_mat, int64_t a_rows, const v
     CUtensorMap tmA, tmB;
     if (make_tmap(&tmA, TM_BF16, GROUPED ? 3 : 2, A_bf16, {K, M, n_mat}, {K * 2, a_rows * K * 2}, {64, BM, 1}, true)) return -10;
     if (make_tmap(&tmB, TM_BF16, 2, B_bf16, {K, N}, {K * 2}, {64, BN}, true)) return -11;
-    if (int rc = opt_in_smem((const void *)k_gemm_bf16<BN, GROUPED>, cfg::SMEM)) return rc;
+    if (!b200q_opt_in_smem((const void *)k_gemm_bf16<BN, GROUPED>, cfg::SMEM)) return -12;
     dim3 grid((unsigned)((M + BM - 1) / BM), row_tiles<BN, GROUPED>(N, n_mat), (unsigned)k_split);
     k_gemm_bf16<BN, GROUPED><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(tmA, tmB, dst, (int)M, (int)N, (int)K, k_split, rt);
     return (int)cudaGetLastError();
@@ -738,7 +726,7 @@ int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const 
     }
     if (make_tmap(&a.tmB, TM_BF16, 2, d.xb, {d.K, d.N}, {d.K * 2}, {64, cfg::BN}, true)) return -11;
     a.n_seg = d.n_seg; a.N = (int)d.N; a.K = (int)d.K; a.k_split = k_split; a.rt = rt;
-    if (int rc = opt_in_smem((const void *)k_gemm_q<TYPE, NB, GROUPED>, cfg::SMEM)) return rc;
+    if (!b200q_opt_in_smem((const void *)k_gemm_q<TYPE, NB, GROUPED>, cfg::SMEM)) return -12;
     dim3 grid((unsigned)tiles, row_tiles<cfg::BN, GROUPED>(d.N, n_mat), (unsigned)k_split);
     k_gemm_q<TYPE, NB, GROUPED><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(a);
     return (int)cudaGetLastError();
@@ -768,7 +756,7 @@ int launch_gemm_bn_i8(const b200q_gemm_multi & d, const int8_t * xq, const float
     }
     if (make_tmap(&a.tmB, TM_U8, 2, xq, {d.K, d.N}, {d.K}, {128, cfg::BN}, true)) return -11;
     a.ts = ts; a.sx = sx; a.n_seg = d.n_seg; a.N = (int)d.N; a.K = (int)d.K; a.k_split = 1;
-    if (int rc = opt_in_smem((const void *)k_gemm_bn_i8<NB>, cfg::SMEM)) return rc;
+    if (!b200q_opt_in_smem((const void *)k_gemm_bn_i8<NB>, cfg::SMEM)) return -12;
     dim3 grid((unsigned)tiles, row_tiles<cfg::BN, false>(d.N, 1), 1);
     k_gemm_bn_i8<NB><<<grid, GEMM_THREADS, cfg::SMEM, st>>>(a);
     return (int)cudaGetLastError();
@@ -794,12 +782,15 @@ int gemmq_choose_split(int64_t tiles, int64_t nr, int sm_count) {
 
 
 // IQ2_BN prefill on the int8 tensor pipe.  X f32 [N][K] is quantised per token into `ws` (int8 [N][K] | ts[N] | sx[N]); up to 3 tensors share it.
-// Requires K % 64 == 0 (16-byte TMA strides); returns -100 when the shape is not eligible (callers use the bf16 path).
+// Eligible shapes (b200q_gemm_bn_i8_ok): K % 64 == 0 (16-byte TMA strides), 16-byte aligned rows of x; callers take the bf16 path for the others.
 size_t b200q_gemm_i8_workspace_bytes(int64_t K, int64_t N) { return (size_t)b200q_align_up(N * K, 256) + (size_t)b200q_align_up(N * 8, 256); }
+bool b200q_gemm_bn_i8_ok(int type, int64_t K, int64_t N, const float * x, int64_t x_stride, size_t ws_bytes) {
+    const int64_t xs = x_stride ? x_stride : K;
+    return type == B200Q_TYPE_IQ2_BN && K % 64 == 0 && N >= 1 && !((uintptr_t)x & 15) && !(xs & 3) && ws_bytes >= b200q_gemm_i8_workspace_bytes(K, N);
+}
 int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t x_stride, void * ws, size_t ws_bytes, cudaStream_t st) {
-    if (d.type != B200Q_TYPE_IQ2_BN || d.K % 64 || d.N < 1 || d.n_seg < 1 || d.n_seg > GEMMQ_MAX_SEGS) return -100;
+    if (!b200q_gemm_bn_i8_ok(d.type, d.K, d.N, x, x_stride, ws_bytes) || d.n_seg < 1 || d.n_seg > GEMMQ_MAX_SEGS) return -2;
     const int64_t xs = x_stride ? x_stride : d.K;
-    if (((uintptr_t)x & 15) || (xs & 3) || ws_bytes < b200q_gemm_i8_workspace_bytes(d.K, d.N)) return -100;
     int8_t * xq = (int8_t *)ws; float * ts = (float *)((char *)ws + b200q_align_up(d.N * d.K, 256)); int * sx = (int *)(ts + d.N);
     k_quantize_rows_i8<<<(unsigned)d.N, 256, 0, st>>>(x, xs, xq, ts, sx, d.K);
     cudaError_t e = cudaGetLastError(); if (e != cudaSuccess) return (int)e;
@@ -941,11 +932,10 @@ int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * d
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
                       void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st) {
     if (ws_bytes < b200q_gemm_workspace_bytes(type, M, K, N)) return -5;
-    if (type == B200Q_TYPE_IQ2_BN && fused) {          // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
+    if (fused && b200q_gemm_bn_i8_ok(type, K, N, x, x_stride, ws_bytes)) {     // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
         b200q_gemm_multi d; memset(&d, 0, sizeof d);
         d.type = type; d.n_seg = 1; d.W[0] = W; d.dst[0] = dst; d.M[0] = M; d.K = K; d.N = N;
-        const int rc = b200q_launch_gemm_bn_i8(d, x, x_stride, ws, ws_bytes, st);
-        if (rc != -100) return rc;
+        return b200q_launch_gemm_bn_i8(d, x, x_stride, ws, ws_bytes, st);
     }
     void * xb = ws;
     void * wb = (char *)ws + b200q_align_up(N * K * 2, 256);

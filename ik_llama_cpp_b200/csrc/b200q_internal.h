@@ -71,7 +71,6 @@ static inline size_t b200q_q8_image_bytes(int64_t k) { return (size_t)(k + 12 * 
 
 int b200q_launch_repack(const void * wire, void * planes, const b200q_layout & L, int inverse, cudaStream_t st);
 int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out, cudaStream_t st);
-int b200q_launch_mmvq(const b200q_mmvq_desc & d, cudaStream_t st);
 // MoE decode: W = n_expert matrices [rows_layout x K], b200q_plane_bytes(type, rows_layout, K) apart; ids device int32 [n_tokens][n_used];
 // x f32 [n_tokens][nb1][K]; dst f32 [n_tokens][n_used][M].  An operand is rows [row0, row0 + M) of its expert matrices: the split form is
 // W_row0 = W2_row0 = 0 with rows_layout = M, merged up/gate experts ([gate; up], rows_layout = 2 M) are W = W2 with W_row0 = M (up), W2_row0 = 0 (gate).
@@ -83,7 +82,6 @@ struct b200q_mmvq_id_desc {
 int b200q_launch_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
 int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
 // wire-layout types (b200q_wire.cu)
-int b200q_launch_wire_mmvq(const b200q_mmvq_desc & d, cudaStream_t st);
 int b200q_launch_wire_dequant_bf16(int type, const void * W, int64_t M, int64_t K, void * out, cudaStream_t st);
 
 // prefill: up to 3 weight tensors of one type / K that share the bf16 activation operand xb [N][K]
@@ -99,6 +97,8 @@ int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * d
 int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_mul_unary(const float * gate, const float * up, float * dst, void * dst_bf16, int64_t total, int act, float limit, cudaStream_t st);
 size_t b200q_gemm_i8_workspace_bytes(int64_t K, int64_t N);
+// IQ2_BN on the int8 tensor pipe: whether the shape is eligible (callers take the bf16 path for the others)
+bool b200q_gemm_bn_i8_ok(int type, int64_t K, int64_t N, const float * x, int64_t x_stride, size_t ws_bytes);
 int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t x_stride, void * ws, size_t ws_bytes, cudaStream_t st);
 int b200q_launch_add_rows(const float * a, const float * b, float * dst, int64_t m, int64_t n, int64_t nb, cudaStream_t st);
 int b200q_launch_f32_to_bf16(const float * x, int64_t x_stride, void * out, int64_t K, int64_t N, cudaStream_t st);

@@ -10,11 +10,10 @@
 #include "b200q_wire.cuh"
 #include "b200q_internal.h"
 #include "b200q_decode_common.cuh"
+#include "b200q_decode_plan.h"
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <string.h>
-
-int b200q_wire_check(int type, int64_t M, int64_t K);
 
 namespace {
 
@@ -100,32 +99,11 @@ __global__ void __launch_bounds__(256) k_wire_mmvq(const wire_mmvq_args a) {
     }
 }
 
-template <int TYPE, int NCOLS, bool UPGATE>
-int launch_wire_mmvq_t(const wire_mmvq_args & a, int sm_count, bool pdl, cudaStream_t st) {
-    const size_t smem = (size_t)NCOLS * a.K + (size_t)NCOLS * (a.K / 32) * 8;
-    static size_t configured[B200Q_MAX_DEVICES] = {};
-    const int dev = b200q_current_device();
-    if (smem > 48 * 1024 && smem > configured[dev]) {
-        if (cudaFuncSetAttribute(k_wire_mmvq<TYPE, NCOLS, UPGATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -3;
-        configured[dev] = smem;
-    }
-    const int nwarps = 8;
-    int64_t grid = (a.M_total + nwarps - 1) / nwarps;
-    const int64_t cap = (int64_t)sm_count * (smem > 100 * 1024 ? 1 : smem > 48 * 1024 ? 2 : 4);
-    if (grid > cap) grid = cap;
-    if (grid < 1) grid = 1;
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(nwarps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    return (int)cudaLaunchKernelEx(&cfg, k_wire_mmvq<TYPE, NCOLS, UPGATE>, a);
-}
-
+// the kernel a plan (plan_mmvq) launches for this type
 template <int TYPE>
-int launch_wire_mmvq_type(const wire_mmvq_args & a, int ncols, bool upgate, int sm_count, bool pdl, cudaStream_t st) {
-#define CASE(N) case N: return upgate ? launch_wire_mmvq_t<TYPE, N, true>(a, sm_count, pdl, st) : launch_wire_mmvq_t<TYPE, N, false>(a, sm_count, pdl, st);
-    switch (ncols) { CASE(1) CASE(2) CASE(4) CASE(8) default: return -2; }
+const void * wire_mmvq_kernel(const b200q_mmvq_plan & p) {
+#define CASE(N) case N: return p.upgate ? (const void *)k_wire_mmvq<TYPE, N, true> : (const void *)k_wire_mmvq<TYPE, N, false>;
+    switch (p.ncols) { CASE(1) CASE(2) CASE(4) CASE(8) default: return nullptr; }
 #undef CASE
 }
 
@@ -175,29 +153,6 @@ __global__ void __launch_bounds__(256) k_wire_mmvq_id(const wire_id_args a) {
         if (lane == 0) a.dst[(int64_t)s * a.M + row] = v;
     }
 }
-template <int TYPE>
-int launch_wire_mmvq_id_t(const wire_id_args & a, bool upgate, int sm_count, bool pdl, cudaStream_t st) {
-    const size_t smem = (size_t)a.ncx * a.K + (size_t)a.ncx * (a.K / 32) * 8;
-    if (smem > 200 * 1024) return -2;
-    static size_t configured[2][B200Q_MAX_DEVICES] = {};
-    const int dev = b200q_current_device();
-    if (smem > 48 * 1024 && smem > configured[upgate][dev]) {
-        const cudaError_t e = upgate ? cudaFuncSetAttribute(k_wire_mmvq_id<TYPE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                     : cudaFuncSetAttribute(k_wire_mmvq_id<TYPE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return -3;
-        configured[upgate][dev] = smem;
-    }
-    const int nwarps = 8;
-    int64_t grid = ((int64_t)a.n_slots * a.M + nwarps - 1) / nwarps; const int64_t cap = (int64_t)sm_count * (smem > 100 * 1024 ? 1 : smem > 48 * 1024 ? 2 : 4);
-    if (grid > cap) grid = cap; if (grid < 1) grid = 1;
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(nwarps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    return upgate ? (int)cudaLaunchKernelEx(&cfg, k_wire_mmvq_id<TYPE, true>, a) : (int)cudaLaunchKernelEx(&cfg, k_wire_mmvq_id<TYPE, false>, a);
-}
-
 }  // namespace
 
 int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
@@ -208,12 +163,16 @@ int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
     a.W = (const uint8_t *)d.W + b200q_row_offset(L, 0, d.W_row0); a.W2 = d.W2 ? (const uint8_t *)d.W2 + b200q_row_offset(L, 0, d.W2_row0) : nullptr;
     a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used;
     a.n_used = d.n_used; a.nb1 = d.nb1; a.ncx = d.n_tokens * d.nb1; a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit;
+    b200q_mmvq_plan p; if (const int prc = b200q_plan_mmvq_id(d, p)) return prc;
+    const void * k = nullptr;
     switch (d.type) {
-#define X(T) case T: return launch_wire_mmvq_id_t<T>(a, d.W2 != nullptr, d.sm_count, d.pdl != 0, st);
+#define X(T) case T: k = p.upgate ? (const void *)k_wire_mmvq_id<T, true> : (const void *)k_wire_mmvq_id<T, false>; break;
         B200Q_FOR_WIRE_TYPES(X)
 #undef X
         default: return -1;
     }
+    if (!b200q_opt_in_smem(k, p.smem)) return -3;
+    return b200q_launch_pdl(k, p.grid, p.block, p.smem, &a, d.pdl != 0, st);
 }
 
 // wire "layout": the tensor is stored verbatim; M must be a multiple of the row interleave
@@ -241,24 +200,21 @@ int b200q_launch_wire_dequant_bf16_experts(int type, const void * W, int64_t M, 
     return (int)cudaGetLastError();
 }
 
-int b200q_launch_wire_mmvq(const b200q_mmvq_desc & d, cudaStream_t st) {
+int b200q_launch_wire_mmvq(const b200q_mmvq_desc & d, const b200q_mmvq_plan & p, cudaStream_t st) {
     wire_mmvq_args a; memset(&a, 0, sizeof a);
-    if (d.n_seg < 1 || d.n_seg > B200Q_MAX_SEGS || d.ncols < 1 || d.ncols > 8) return -2;
-    if (d.tp.in || d.tp.out) return -7;
-    if (d.q8_in || d.q8_out) return -8;
     int64_t r0 = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        const int rc = b200q_wire_check(d.type, d.seg[i].M, d.K); if (rc) return rc;
         a.W[i] = (const uint8_t *)d.seg[i].W; a.dst[i] = d.seg[i].dst; a.bias[i] = d.seg[i].bias; a.M[i] = d.seg[i].M; a.row0[i] = r0; r0 += d.seg[i].M;
     }
     a.W2 = (const uint8_t *)d.seg[0].W2;
     a.n_seg = d.n_seg; a.M_total = r0; a.K = d.K; a.x = d.x; a.x_stride = d.x_stride ? d.x_stride : d.K; a.act = d.act; a.limit = d.limit;
-    const bool upgate = d.seg[0].W2 != nullptr;
-    if (upgate && d.n_seg != 1) return -2;
+    const void * k = nullptr;
     switch (d.type) {
-#define X(T) case T: return launch_wire_mmvq_type<T>(a, d.ncols, upgate, d.sm_count, d.pdl != 0, st);
+#define X(T) case T: k = wire_mmvq_kernel<T>(p); break;
         B200Q_FOR_WIRE_TYPES(X)
 #undef X
         default: return -1;
     }
+    if (!b200q_opt_in_smem(k, p.smem)) return -3;
+    return b200q_launch_pdl(k, p.grid, p.block, p.smem, &a, d.pdl != 0, st);
 }

@@ -1,11 +1,12 @@
-"""Element-by-element tests of every decode mat-vec schedule (n <= 8).  The dispatcher picks the launch from the shape:
-  * mmvq_cols (b200q_api.cu) covers n with pieces of 8, 4, 2 and 1 columns, halving a piece while c K 1.25 bytes exceed 200 KB;
-  * pieces of 1 or 2 columns take the TMA-ring kernel k_mmvq_ring<T, NCOLS, UPGATE, MULTI, PAIR, TP, Q8> (b200q_decode_ring.cuh) unless a plane
+"""Element-by-element tests of every decode mat-vec schedule (n <= 8).  The host plans each launch from the shape before it launches it:
+  * mmvq_cols (b200q_api.cu) covers n with pieces of 8, 4, 2 and 1 columns, halving a piece while c K 1.25 bytes exceed 200 KB (b200q_mmvq_max_cols);
+  * plan_mmvq (b200q_decode.cu) picks the kernel, its template arguments, grid and block of each piece: pieces of 1 or 2 columns take the
+    TMA-ring kernel k_mmvq_ring<T, NCOLS, UPGATE, MULTI, PAIR, TP, Q8> (b200q_decode_ring.cuh) unless a plane
     row is not 16-byte aligned (make_ring_geom), ring_shape finds no layout with 2 stages at 11, 7 or 3 consumer warps, or a row-pair launch has an
     odd segment that is not the last; pieces of 4 or 8 columns and those fallbacks take the LDG kernel k_mmvq<T, NCOLS, UPGATE>;
   * K <= 4096: a ring unit is a pair of rows (PAIR); K > 4096: one row cut into segments of up to 256 items ("long rows"), halves of 128 items;
   * the q8 hand-off: the up/gate launch emits its result as a q8_1 image (Q8 = 2), the next launch consumes it (Q8 = 1); shapes that are not eligible
-    retry as plain launches;
+    are planned as plain launches;
   * wire-layout types take k_wire_mmvq<T, NCOLS, UPGATE> (b200q_wire.cu).
 The table below names, per case, the launches it is meant to reach; each case runs once under torch.profiler in a child process of its own and the
 trace must show exactly those launches (kernel, template arguments, grid, block) at 132 SMs.  On another SM count, or when the profiler records no

@@ -228,7 +228,13 @@ int b200q_mul_mat_vec_q8(int type, const void * W, const float * x, const void *
 int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const void * W_gate, float * const * dst, const int64_t * m,
                          int64_t k, const float * x, int unary, float limit, const b200q_nvls_comm * comm, int reduce_in, int reduce_out, void * stream) {
     if (n_tensors < 1 || n_tensors > B200Q_MAX_SEGS || !W || !m || (W_gate && n_tensors != 1)) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: bad argument");
-    if ((reduce_in || reduce_out) && (!comm || !comm->ll_mc || !comm->ll_local || !comm->ll_reduced || !comm->ll_state || comm->ll_stride < 1 || comm->world_size < 2 || comm->rank >= comm->world_size
+    // the sum over ranks of unary(gate . x) * (up . x) means nothing: a fused up/gate launch may consume a reduce, never produce one
+    if (W_gate && reduce_out) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: a fused up/gate launch cannot reduce_out");
+    // unicast variant (peer stores, rows of a CTA coalesced): measured slower than the multicast stores at 2 GPUs -> opt-in only.  Only then may
+    // ll_mc be NULL: no launch ever issues multimem.st to an address that is not a multicast mapping.
+    static const int ucast_env = [] { const char * e = getenv("B200Q_TP_UNICAST"); return e ? atoi(e) : 0; }();
+    const bool ucast = ucast_env && comm && comm->ll_peers && comm->world_size <= 8;
+    if ((reduce_in || reduce_out) && (!comm || (!comm->ll_mc && !ucast) || !comm->ll_local || !comm->ll_reduced || !comm->ll_state || comm->ll_stride < 1 || comm->world_size < 2 || comm->rank >= comm->world_size
                                       || ((uintptr_t)comm->ll_mc & 15) || ((uintptr_t)comm->ll_local & 15) || ((uintptr_t)comm->ll_reduced & 15) || (comm->ll_stride & 1)))
         return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: incomplete communicator");
     if (!reduce_in && !x) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: x is NULL");
@@ -240,9 +246,7 @@ int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const 
     if (comm) {
         d.tp.ll_mc = (float2 *)comm->ll_mc; d.tp.ll_local = (const float2 *)comm->ll_local; d.tp.ll_red = (float2 *)comm->ll_reduced; d.tp.ll_stride = comm->ll_stride;
         d.tp.world = comm->world_size; d.tp.rank = comm->rank; d.tp.seq = (uint32_t *)comm->ll_state; d.tp.in = reduce_in != 0; d.tp.out = reduce_out != 0;
-        // unicast variant (peer stores, rows of a CTA coalesced): measured slower than the multicast stores at 2 GPUs -> opt-in only
-        static const int ucast = [] { const char * e = getenv("B200Q_TP_UNICAST"); return e ? atoi(e) : 0; }();
-        if (ucast && comm->ll_peers && comm->world_size <= 8) {
+        if (ucast) {
             for (uint32_t r = 0; r < comm->world_size; ++r) {
                 if (!comm->ll_peers[r] || ((uintptr_t)comm->ll_peers[r] & 15)) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: bad peer mapping");
                 d.tp.ll_peer[r] = (float2 *)comm->ll_peers[r];

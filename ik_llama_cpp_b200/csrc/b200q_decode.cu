@@ -226,7 +226,7 @@ static int plan_mmvq(const b200q_mmvq_desc & d, b200q_mmvq_plan & p) {
     for (int i = 0; i < d.n_seg; ++i) M_total += d.seg[i].M;
     p.ncols = d.ncols; p.upgate = upgate;
     if (b200q_is_wire_type(d.type)) {                       // k_wire_mmvq: 8 warps, a warp per row
-        if (tp) return -7;
+        if (tp) return -1;                                  // the fused reduce exists only in the ring kernel of the plane types
         for (int i = 0; i < d.n_seg; ++i) if (const int rc = b200q_wire_check(d.type, d.seg[i].M, d.K)) return rc;
         if ((upgate && d.n_seg != 1) || !ldg_cols) return -2;
         p.kernel = B200Q_MMVQ_WIRE; p.smem = b200q_mmvq_x_bytes(d.ncols, d.K);
@@ -234,8 +234,8 @@ static int plan_mmvq(const b200q_mmvq_desc & d, b200q_mmvq_plan & p) {
         return 0;
     }
     for (int i = 0; i < d.n_seg; ++i) { b200q_layout L; if (const int rc = b200q_make_layout(d.type, d.seg[i].M, d.K, &L)) return rc; }
-    // only the TMA-ring kernel implements the fused reduce
-    if (tp && (d.ncols != 1 || !d.ring || d.K % 256 || (d.tp.out && M_total > d.tp.ll_stride) || (d.tp.in && d.K > d.tp.ll_stride))) return -7;
+    // only the TMA-ring kernel implements the fused reduce: every other case is a shape error
+    if (tp && (d.ncols != 1 || !d.ring || d.K % 256 || (d.tp.out && M_total > d.tp.ll_stride) || (d.tp.in && d.K > d.tp.ll_stride))) return -2;
     // q8 hand-off: n = 1, single tensor, ring kernel, bulk-copyable image; the up/gate launch emits it (q8 = 2), a plain launch consumes it (q8 = 1)
     const bool q8_ok = d.ncols == 1 && d.n_seg == 1 && d.ring && !tp
                     && (!d.q8_in || (d.K % 64 == 0 && !((uintptr_t)d.q8_in & 15)))
@@ -243,7 +243,7 @@ static int plan_mmvq(const b200q_mmvq_desc & d, b200q_mmvq_plan & p) {
     p.q8 = !q8_ok ? 0 : d.q8_out ? 2 : d.q8_in && !upgate ? 1 : 0;
     p.multi = !upgate && d.n_seg > 1; p.tp = tp;
     if (d.ring && d.ncols <= 2 && plan_ring(d, M_total, p)) return 0;
-    if (tp) return -7;
+    if (tp) return -2;                                      // no ring geometry for this (type, K) or ring layout for this shape
     p.multi = p.tp = false; p.q8 = 0;
     if (!ldg_cols) return -2;
     // k_mmvq: one warp per row, one CTA per SM; shrink the CTA when there are fewer rows than warps

@@ -137,15 +137,25 @@ B200Q_API int b200q_reduce_sum_nvls_bf16(const float * in, float * out_f32, void
  * 8-byte store.  reduce_out: the kernel's epilogue broadcasts each finished partial row to slot [parity][this rank][row] of EVERY rank with
  * multimem.st through the NVLS multicast mapping (dst is not written; m_total <= ll_stride).  reduce_in: `x` is ignored; the CTAs of the consumer
  * sum the per-rank slots in rank order (bit-identical on every rank), each its own slice, publish the sums in ll_reduced with the same tagging and
- * quantise their activations from there (k <= ll_stride).  W_gate != NULL: fused up/gate mode (n_tensors = 1).
+ * quantise their activations from there (k <= ll_stride).  W_gate != NULL: fused up/gate mode (n_tensors = 1), reduce_in only: a fused up/gate
+ * launch with reduce_out returns B200Q_E_ARG (the sum over ranks of unary(gate . x) * (up . x) is not a result of anything).
  * CONTRACT: on one communicator every reduce_out launch must be followed, on every rank, by at least one reduce_in launch before the next
  * reduce_out (the two parities are reused every second reduce); all ranks issue the same sequence.
- *   ll_mc / ll_local: multicast / local address of the symmetric slot array, 2 * world_size * ll_stride entries of 8 bytes, zero-initialised;
+ * Launches with reduce_in or reduce_out run on the ring kernel only, so they are accepted exactly when a plain n = 1 b200q_mul_mat_vec /
+ * _multi / b200q_fused_up_gate_vec of the same tensors is planned on the ring kernel and:
+ *   - type is a plane-layout type: a wire-layout type returns B200Q_E_TYPE;
+ *   - k % 256 == 0, m_total = sum of m <= ll_stride for reduce_out, k <= ll_stride for reduce_in: otherwise B200Q_E_SHAPE;
+ *   - the type has a ring geometry at this k (every plane row 16-byte aligned, e.g. Q6_K needs k % 2048 == 0), and on row pairs (k <= 4096)
+ *     every tensor but the last has an even m: otherwise B200Q_E_SHAPE.
+ * A rejected call writes nothing.
+ *   ll_mc / ll_local: multicast / local address of the symmetric slot array, 2 * world_size * ll_stride entries of 8 bytes, zero-initialised.
+ *   ll_mc may be NULL only when the unicast stores are selected (B200Q_TP_UNICAST=1 and ll_peers given); otherwise NULL is B200Q_E_ARG;
  *   ll_reduced: rank-local, 2 * ll_stride entries, zero-initialised; ll_state: rank-local u32[2], zero-initialised; all 16-byte aligned. */
 typedef struct b200q_nvls_comm {
     void * ll_mc; const void * ll_local; void * ll_reduced; int64_t ll_stride; uint32_t world_size; uint32_t rank; void * ll_state;
     void * const * ll_peers;    /* optional (HOST array of world_size device pointers, world_size <= 8): every rank's mapping of the slot array in THIS
-                                 * rank's address space (peer memory).  When given, reduce_out writes each peer's copy with ordinary stores, the rows of
+                                 * rank's address space (peer memory).  When given and B200Q_TP_UNICAST=1 (opt-in, read once per process),
+                                 * reduce_out writes each peer's copy with ordinary stores, the rows of
                                  * a CTA as consecutive 16-byte lanes of one warp (coalesced into 128-byte NVLink packets), instead of one multicast
                                  * store per row pair.  NULL: multimem.st only. */
 } b200q_nvls_comm;

@@ -27,7 +27,8 @@ seventh of the bar.  test_f32_kernel_order_stays_inside_the_bar replays both sum
 The worst case without cancellation, gamma_{L+7} sum |v_i|, would exceed the bar at that K; it is not the case the data can produce.
 
 The MoE mat-vecs (k_mmvq_id, k_wire_mmvq_id, skipped slots included) have their own table and sweep in test_gpu_moe_decode.py, which reuses the
-bars, the profiler and the child-process runner of this file; the tensor-parallel instantiations are covered in test_gpu_tp.py.
+bars, the profiler and the child-process runner of this file.  The tensor-parallel instantiations (TP = true) are covered on one GPU, every
+plane type with W emulated ranks, in test_gpu_tp_decode.py; test_gpu_tp.py runs the fused exchange across real GPUs where the machine has them.
 """
 import json
 import os

@@ -366,6 +366,60 @@ def moe_up_gate_merged(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, unar
     return dst
 
 
+def moe_combine(rows: torch.Tensor, weights: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+    """GGML_OP_MUL_MULTI_ADD (b200q_moe_combine): rows f32 [n_tokens, n_used, M], weights f32 [n_tokens, n_used] -> dst f32 [n_tokens, M],
+    dst[t] = sum_u weights[t, u] * rows[t, u], summed in slot order in f32 as the reference CPU op."""
+    _require_cuda()
+    assert rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 3 and rows.is_contiguous()
+    n_tokens, n_used, m = rows.shape
+    assert weights.is_cuda and weights.dtype == torch.float32 and weights.is_contiguous() and weights.numel() == n_tokens * n_used
+    dst = out if out is not None else torch.empty((n_tokens, m), dtype=torch.float32, device=rows.device)
+    assert dst.dtype == torch.float32 and dst.is_contiguous() and dst.numel() == n_tokens * m
+    with torch.cuda.device(rows.device):
+        check(_lib.lib().b200q_moe_combine(rows.data_ptr(), weights.data_ptr(), dst.data_ptr(), m, n_used, n_tokens, _stream()), "b200q_moe_combine")
+    return dst
+
+
+@dataclass
+class SharedExpert:
+    """One rank's shard of a dense shared expert (ffn_up_shexp / ffn_gate_shexp rows, ffn_down_shexp K range), as tp.shard_rows / shard_cols cut
+    them.  None on a rank whose shard is empty."""
+    up: QuantTensor
+    gate: QuantTensor
+    down: QuantTensor
+
+
+def moe_tp_partial(x: torch.Tensor, ids: torch.Tensor, weights: torch.Tensor, n_embd: int, down: "ExpertTensor | None",
+                   up: "ExpertTensor | None" = None, gate: "ExpertTensor | None" = None, gate_up: "ExpertTensor | None" = None,
+                   shared: "SharedExpert | None" = None, unary: str = "silu", limit: float = 0.0) -> torch.Tensor:
+    """One rank's partial of a MoE FFN under tensor parallelism (per device in the reference: llm_build_moe_ffn on the shards, + the shared
+    expert's output, src/llama-build-context.cpp:1894-1976).  x f32 [n_tokens, K] (replicated), ids int32 [n_tokens, n_used], weights f32
+    [n_tokens, n_used] -> f32 [n_tokens, n_embd]:
+        up/gate of the rank's expert rows (split up / gate, or merged gate_up) -> ffn_down_exps K shard (mul_mat_id_dispatch) -> moe_combine,
+        plus the shared expert's row-parallel partial if given (fused into the down mat-vec as its bias at one token, an add_rows otherwise).
+    down None: the rank's routed shard is empty (tp.moe_ffn_plan gave it 0 rows) and contributes zeros.  Summing the partials over the ranks
+    is the caller's reduce (NvlsReducer.all_reduce for decode, all_reduce_bf16 for prefill)."""
+    _require_cuda()
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()
+    n_tokens = x.shape[0]
+    if down is None:
+        routed = torch.zeros((n_tokens, n_embd), dtype=torch.float32, device=x.device)
+    else:
+        assert down.m == n_embd and (gate_up is None) == (up is not None)
+        x3 = x.view(n_tokens, 1, x.shape[1])
+        par = moe_up_gate_merged(gate_up, x3, ids, unary, limit) if gate_up is not None else mul_mat_id_dispatch(up, x3, ids, gate=gate, unary=unary, limit=limit)
+        routed = moe_combine(mul_mat_id_dispatch(down, par, ids), weights)
+    if shared is None:
+        return routed
+    h = fused_up_gate(shared.up, shared.gate, x, unary)
+    if n_tokens == 1:
+        return mul_mat(shared.down, h, bias=routed.view(-1))
+    s = mul_mat(shared.down, h)
+    with torch.cuda.device(x.device):
+        check(_lib.lib().b200q_add_rows(s.data_ptr(), routed.data_ptr(), s.data_ptr(), n_embd, n_tokens, n_tokens, _stream()), "b200q_add_rows")
+    return s
+
+
 def dequantize_bf16(w: QuantTensor) -> torch.Tensor:
     _require_cuda()
     out = torch.empty((w.m, w.k), dtype=torch.bfloat16, device=w.planes.device)

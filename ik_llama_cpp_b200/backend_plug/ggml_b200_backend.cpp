@@ -2,7 +2,8 @@
 //
 // Implements the reference's backend vtable (struct ggml_backend_i, ggml/src/ggml-backend-impl.h:81-130) and buffer vtables
 // (:18-51) on top of libb200q.so, and exports the C symbols of ggml/include/ggml-cuda.h:24-46 under their original names.
-// graph_compute owns the hot path: GGML_OP_MUL_MAT on block-quantized src0 (2-D and batched), GGML_OP_FUSED_UP_GATE, the look-ahead
+// graph_compute owns the hot path: GGML_OP_MUL_MAT on block-quantized src0 (2-D and batched), GGML_OP_FUSED_UP_GATE, the MoE ops (MUL_MAT_ID,
+// MOE_FUSED_UP_GATE and the MUL_MULTI_ADD that combines the routed experts, so a MoE FFN never leaves the device), the look-ahead
 // fusions of ggml_cuda_mul_mat_q (Q,K,V sharing src1; a trailing bias ADD, ggml-cuda.cu:2573-2601) and the q8_1 hand-off from
 // FUSED_UP_GATE to the following MUL_MAT (ffn_down).  Every other op is reported as unsupported (supports_op == false): this library is the
 // quantized-mat-mul backend; the pass-through kernels (norm, rope, attention ...) of a full llama graph are outside SURVEY §8a.
@@ -291,6 +292,14 @@ GGML_CALL static bool b200_backend_supports_op(ggml_backend_t, const ggml_tensor
             if (op->type != GGML_TYPE_F32 || !ggml_is_contiguous(op) || w->ne[0] != x->ne[0] || x->ne[3] != 1 || ids->ne[1] != x->ne[2] || ids->ne[0] % x->ne[1]) return false;
             return x->ne[1] * (w->ne[0] + w->ne[0] / 4) <= 200 * 1024;      // one token's columns must fit
         }
+        case GGML_OP_MUL_MULTI_ADD: {
+            // the routing-weighted sum that ends llm_build_moe_ffn under fused_mmad: experts f32 [m, n_used, n_tokens], weights f32 [1, n_used, n_tokens];
+            // the scales form (src[2] / src[3]: down_exps_s) stays on the CPU
+            const ggml_tensor * e = op->src[0]; const ggml_tensor * w = op->src[1];
+            return e && w && !op->src[2] && !op->src[3] && e->type == GGML_TYPE_F32 && w->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32 &&
+                   ggml_is_contiguous(e) && ggml_is_contiguous(w) && ggml_is_contiguous(op) && e->ne[3] == 1 && w->ne[0] == 1 && w->ne[1] == e->ne[1] &&
+                   w->ne[2] == e->ne[2] && w->ne[3] == 1 && op->ne[0] == e->ne[0] && op->ne[1] == e->ne[2] && op->ne[2] == 1 && op->ne[3] == 1;
+        }
         case GGML_OP_FUSED_UP_GATE:
             return op->src[0] && op->src[1] && !op->src[3] && !op->src[4] && op->src[0]->type == op->src[1]->type && op->src[2] && op->src[2]->ne[2] * op->src[2]->ne[3] == 1 &&
                    op->src[0]->ne[2] == 1 && op->src[1]->ne[2] == 1 && b200_can_mul_mat(op->src[0], op->src[2], op) &&
@@ -386,6 +395,10 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
                                                                  node->ne[0], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], unary, limit, ws, need, c->stream));
                 else B200Q_CHECK(b200q_mul_mat_id(w->type, w->data, g ? g->data : nullptr, (int)w->ne[2], id, (const float *)x->data, (float *)node->data,
                                                   w->ne[1], w->ne[0], (int)ids->ne[0], (int)x->ne[1], (int)x->ne[2], unary, limit, ws, need, c->stream));
+            } break;
+            case GGML_OP_MUL_MULTI_ADD: {
+                const ggml_tensor * e = node->src[0];
+                B200Q_CHECK(b200q_moe_combine((const float *)e->data, (const float *)node->src[1]->data, (float *)node->data, e->ne[0], (int)e->ne[1], (int)e->ne[2], c->stream));
             } break;
             case GGML_OP_FUSED_UP_GATE: {
                 const ggml_tensor * up = node->src[0]; const ggml_tensor * gate = node->src[1]; const ggml_tensor * x = node->src[2];

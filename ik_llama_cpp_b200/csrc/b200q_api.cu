@@ -469,6 +469,15 @@ int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_expert, con
         return moe_vec(type, o, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, stream, what);
     return moe_gemm(type, o, n_expert, ids, x, dst, m, k, n_used, nb1, n_tokens, unary, limit, workspace, workspace_bytes, stream, what);
 }
+int b200q_moe_combine(const float * rows, const float * weights, float * dst, int64_t m, int n_used, int n_tokens, void * stream) {
+    static const char * what = "b200q_moe_combine";
+    if (!rows || !weights || !dst || ((uintptr_t)rows & 3) || ((uintptr_t)weights & 3) || ((uintptr_t)dst & 3)) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    if (m < 1 || n_used < 1 || n_tokens < 1 || m > INT64_MAX / ((int64_t)n_used * n_tokens * 4)) return fail(B200Q_E_SHAPE, "%s: bad shape", what);
+    const uintptr_t d0 = (uintptr_t)dst, d1 = d0 + (uintptr_t)(m * n_tokens * 4);
+    const uintptr_t r0 = (uintptr_t)rows, r1 = r0 + (uintptr_t)(m * n_used * n_tokens * 4), w0 = (uintptr_t)weights, w1 = w0 + (uintptr_t)n_used * n_tokens * 4;
+    if ((d0 < r1 && r0 < d1) || (d0 < w1 && w0 < d1)) return fail(B200Q_E_ARG, "%s: dst overlaps an input", what);
+    return check_launch(b200q_launch_moe_combine(rows, weights, dst, m, n_used, n_tokens, (cudaStream_t)stream), what);
+}
 int b200q_mul_mat_host(int type, const void * W, const float * x_host, float * dst_host, int64_t m, int64_t k, int64_t n, void * stream) {
     cudaStream_t st = (cudaStream_t)stream; cudaError_t e; int rc;
     const size_t xb = (size_t)n * k * sizeof(float), yb = (size_t)n * m * sizeof(float), wsb = b200q_mul_mat_workspace(type, m, k, n);

@@ -124,6 +124,8 @@ int b200q_launch_wire_dequant_bf16_experts(int type, const void * W, int64_t M, 
 int b200q_moe_gemm_shape_ok(int type, int64_t M, int64_t K, int n_used, int nb1, int n_tokens, int n_expert, int up_gate);
 size_t b200q_moe_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_slots, int n_expert, int up_gate, int64_t rows_layout);
 int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_bytes, cudaStream_t st);
+// GGML_OP_MUL_MULTI_ADD: dst f32 [n_tokens][m] = sum over u of w[t][u] * rows[t][u][:] (arguments checked by the caller)
+int b200q_launch_moe_combine(const float * rows, const float * w, float * dst, int64_t m, int n_used, int n_tokens, cudaStream_t st);
 
 // row origins of the MoE operands (b200q_mmvq_id_desc, b200q_moe_gemm), resolved on the host: bytes from the start of plane p to row `row0`
 // (wire-layout types: of the verbatim tensor, row0 a multiple of the row interleave); rows [row0, ...) of a tensor then read like a tensor of

@@ -12,6 +12,9 @@
 //   4. up/gate: up and gate are two segments of that launch (up -> workspace, gate -> dst), then k_mul_unary over n_slots x M.  Merged up/gate
 //      experts ([gate; up] in one [2 M x K] matrix per expert) are the same two segments over row ranges of one tensor (b200q_moe_gemm::row0).
 // The reference's generic path (ggml_cuda_mul_mat_id, ggml-cuda.cu:2836-2950) copies ids to the host and synchronises to build its row mapping.
+//
+// k_moe_combine: GGML_OP_MUL_MULTI_ADD, the routing-weighted sum over the n_used slots of a token that ends every MoE FFN (and, under tensor
+// parallelism, produces a rank's partial of it).
 #include "b200q_internal.h"
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -85,7 +88,38 @@ moe_ws_layout moe_layout(int type, int64_t M, int64_t K, int64_t n_slots, int n_
     return L;
 }
 
+// dst[t][i] = sum_u w[t][u] * rows[t][u][i] in slot order with the association of the reference CPU op (iqk_mul_multi_add: y = x0 w0, then
+// y = y + x_u w_u), every product and sum rounded on its own (no FMA contraction): bit-equal to the same loop in f32 on the host.
+// T = float4: m % 4 == 0 and 16-byte aligned rows / dst, one 16-byte load per slot and one 16-byte store; T = float otherwise.
+__device__ __forceinline__ float comb_mul(float a, float s) { return __fmul_rn(a, s); }
+__device__ __forceinline__ float4 comb_mul(float4 a, float s) { return make_float4(__fmul_rn(a.x, s), __fmul_rn(a.y, s), __fmul_rn(a.z, s), __fmul_rn(a.w, s)); }
+__device__ __forceinline__ float comb_add(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float4 comb_add(float4 a, float4 b) { return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w)); }
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_moe_combine(const T * __restrict__ rows, const float * __restrict__ w, T * __restrict__ dst, int64_t mv, int n_used, int64_t total) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t t = i / mv, c = i - t * mv;
+        const T * r = rows + t * n_used * mv + c;
+        const float * wt = w + t * n_used;
+        T y = comb_mul(__ldg(r), __ldg(wt));
+#pragma unroll 8
+        for (int u = 1; u < n_used; ++u) y = comb_add(y, comb_mul(__ldg(r + u * mv), __ldg(wt + u)));
+        dst[i] = y;
+    }
+}
+
 }  // namespace
+
+int b200q_launch_moe_combine(const float * rows, const float * w, float * dst, int64_t m, int n_used, int n_tokens, cudaStream_t st) {
+    const bool v4 = m % 4 == 0 && !((uintptr_t)rows & 15) && !((uintptr_t)dst & 15);
+    const int64_t mv = v4 ? m / 4 : m, total = mv * n_tokens;
+    const int64_t g = std::min<int64_t>((total + 255) / 256, 132 * 16);
+    if (v4) k_moe_combine<float4><<<(unsigned)g, 256, 0, st>>>((const float4 *)rows, w, (float4 *)dst, mv, n_used, total);
+    else k_moe_combine<float><<<(unsigned)g, 256, 0, st>>>(rows, w, dst, mv, n_used, total);
+    return (int)cudaGetLastError();
+}
 
 // shapes the grouped path takes: K a multiple of 256 (the fused kernel's raw blocks, 16-byte TMA strides), a type the layout supports, at most
 // 1024 experts (one routing thread each); for up/gate n_slots * M a multiple of 4 (the vectorised unary-mul tail)

@@ -6,7 +6,10 @@ ggml/src/ggml-cuda.cu:1003-1192):
   * split_dim = 1 (rows of W: wq/wk/wv/ffn_up/ffn_gate/output): shard = contiguous row range, no exchange;
   * split_dim = 0 (columns/K of W: wo/ffn_down): shard = K range (multiple of the granularity, >= quant block) of EVERY row,
     partial outputs are summed across ranks (GGML_OP_REDUCE, ggml-cuda/reduce.cu:125);
-  * per-row headers (row_meta_size: IQ4_KS, IQ2_BN, ...) are replicated into every K-shard.
+  * per-row headers (row_meta_size: IQ4_KS, IQ2_BN, ...) are replicated into every K-shard;
+  * MoE experts (src/llama-load-tensors.cpp:5637-5675): one n_ff split for the three expert tensors, rows of every ffn_up_exps / ffn_gate_exps
+    matrix (merged ffn_gate_up_exps: the gate rows and the up rows of the same range), the K range of every ffn_down_exps matrix; each rank's
+    routed-expert partial is backend.moe_tp_partial.
 Pure numpy: usable in CPU tests with the oracle as the compute stand-in, and by bench.py / the backend for real shards.
 """
 from __future__ import annotations
@@ -68,6 +71,49 @@ def shard_cols(wire: np.ndarray, ggml_type: int, m: int, k: int, world: int, ran
     out[:, :il * meta] = w[:, :il * meta]
     out[:, il * meta:] = w[:, il * (meta + (k0 // qk) * bs): il * (meta + ((k0 + ks) // qk) * bs)]
     return out.reshape(-1), ks, k0
+
+
+def moe_expert_granularity(down_type: int) -> int:
+    """Unit of the routed experts' n_ff split: 16, or the block size of ffn_down_exps' type if larger (src/llama-load-tensors.cpp:5643-5648)."""
+    return max(16, GEOM[down_type][0])
+
+
+def moe_ffn_plan(n_ff_exp: int, world: int, down_type: int) -> list[int]:
+    """n_ff shard of the routed experts on each rank: rows of ffn_up_exps / ffn_gate_exps, the K range of ffn_down_exps (one split serves all
+    three, src/llama-load-tensors.cpp:5637-5675).  A rank may get 0 (Qwen3-30B-A3B: 768 = 3 x 256 over 8 ranks).  The reference skips such a
+    device; here every rank still joins the reduce, with a zero partial.  The reference also weighs each device's memory already in use
+    (create_split's mem_used); this plan assumes equal use and keeps create_split's rule above."""
+    return create_split(n_ff_exp, moe_expert_granularity(down_type), world)
+
+
+def _expert_rows(wire: np.ndarray, ggml_type: int, n_expert: int, m: int, k: int, ranges) -> np.ndarray:
+    """the rows [a, b) of each range, in order, of every expert matrix [m x k] (whole wire rows; for _R4 types a, b are multiples of 4)"""
+    il = INTERLEAVE.get(ggml_type, 1)
+    assert all(a % il == 0 and b % il == 0 for a, b in ranges)
+    w = np.ascontiguousarray(wire, np.uint8).reshape(n_expert, m, row_size(ggml_type, k))
+    return np.ascontiguousarray(np.concatenate([w[:, a:b] for a, b in ranges], axis=1)).reshape(-1)
+
+
+def shard_expert_rows(wire: np.ndarray, ggml_type: int, n_expert: int, n_ff: int, k: int, split: list[int], rank: int):
+    """ffn_up_exps / ffn_gate_exps [n_expert][n_ff x k] (split_dim 1): rows [r0, r1) of every expert.  Returns (shard_bytes, n_ff_shard)."""
+    r0 = sum(split[:rank]); n = split[rank]
+    return _expert_rows(wire, ggml_type, n_expert, n_ff, k, [(r0, r0 + n)]), n
+
+
+def shard_expert_gate_up(wire: np.ndarray, ggml_type: int, n_expert: int, n_ff: int, k: int, split: list[int], rank: int):
+    """ffn_gate_up_exps [n_expert][2 n_ff x k], gate rows first: gate rows [r0, r1) then up rows [n_ff + r0, n_ff + r1) of every expert
+    (prepare_up_gate_split, src/llama-load-tensors.cpp:4851-4867), again a merged [2 n_ff_shard x k] matrix per expert.
+    Returns (shard_bytes, n_ff_shard)."""
+    r0 = sum(split[:rank]); n = split[rank]
+    return _expert_rows(wire, ggml_type, n_expert, 2 * n_ff, k, [(r0, r0 + n), (n_ff + r0, n_ff + r0 + n)]), n
+
+
+def shard_expert_cols(wire: np.ndarray, ggml_type: int, n_expert: int, m: int, n_ff: int, split: list[int], rank: int):
+    """ffn_down_exps [n_expert][m x n_ff] (split_dim 0): the K range [k0, k1) of every row of every expert, row headers replicated (as
+    shard_cols on the n_expert * m rows).  `split` is moe_ffn_plan's for this type.  Returns (shard_bytes, k_shard, k0)."""
+    out, ks, k0 = shard_cols(wire, ggml_type, n_expert * m, n_ff, len(split), rank, granularity=moe_expert_granularity(ggml_type))
+    assert (ks, k0) == (split[rank], sum(split[:rank])), "ffn_down_exps follows its own type's plan"
+    return out, ks, k0
 
 
 def llama_layer_plan(n_embd: int, n_ff: int, n_head: int, n_head_kv: int, world: int, ggml_type: int):

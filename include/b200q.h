@@ -207,6 +207,15 @@ B200Q_API int b200q_mul_mat_id(int type, const void * W, const void * W_gate, in
 B200Q_API size_t b200q_moe_up_gate_merged_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert);
 B200Q_API int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_expert, const int32_t * ids, const float * x, float * dst,
                              int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
+/* ---- MoE combine: GGML_OP_MUL_MULTI_ADD without the scales form (src[2] / src[3]) ----
+ * (the last node of llm_build_moe_ffn under fused_mmad, src/llama-build-context.cpp:1667-1680; CPU iqk_mul_multi_add, iqk_cpu_ops.cpp:430-495;
+ * CUDA ggml-cuda/multiadd.cu:40-62).  rows f32 [n_tokens][n_used][m] (the MUL_MAT_ID result of ffn_down_exps), weights f32 [n_tokens][n_used] (the
+ * routing weights), dst f32 [n_tokens][m]:  dst[t][i] = sum_u weights[t][u] * rows[t][u][i], summed in slot order as the CPU op (y = x0 w0, then
+ * y = y + x_u w_u) with every product and sum rounded on its own: bit-equal to that loop in f32.  Under tensor parallelism, a rank's rows are its
+ * K-shard of ffn_down_exps and dst is the rank's partial of the layer, summed across ranks by the caller's reduce.  Slots of ids outside the expert
+ * range need no care: MUL_MAT_ID gives them zero rows.  All pointers 4-byte aligned; dst must not overlap rows or weights (B200Q_E_ARG).
+ * Writes only dst; no workspace, allocation or synchronisation (capturable). */
+B200Q_API int b200q_moe_combine(const float * rows, const float * weights, float * dst, int64_t m, int n_used, int n_tokens, void * stream);
 /* same through HOST activations/results: H2D(x) -> mul_mat -> D2H(dst), synchronous (end-to-end entry point) */
 B200Q_API int b200q_mul_mat_host(int type, const void * W_planes_dev, const float * x_host, float * dst_host,
                        int64_t m, int64_t k, int64_t n, void * stream);

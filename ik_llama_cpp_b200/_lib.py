@@ -90,6 +90,10 @@ def lib() -> ctypes.CDLL:
         L.b200q_moe_up_gate_merged.argtypes = [i32, vp, i32, vp, vp, vp, i64, i64, i32, i32, i32, i32, c_float, vp, c_size_t, vp]
     if hasattr(L, "b200q_moe_combine"):
         L.b200q_moe_combine.argtypes = [vp, vp, vp, i64, i32, i32, vp]
+    if hasattr(L, "b200q_mul_mat_batched"):
+        L.b200q_mul_mat_batched_workspace.restype = c_size_t
+        L.b200q_mul_mat_batched_workspace.argtypes = [i32, i64, i64, i64, i32, i32, i64, i64]
+        L.b200q_mul_mat_batched.argtypes = [i32, vp, i32, vp, i64, i64, vp, i64, i64, i64, i32, vp, c_size_t, vp]
     if hasattr(L, "b200q_decode_prefetch_next"):
         L.b200q_decode_prefetch_next.argtypes = [i32, i32, vp, vp, vp, i64]
     _lib = L

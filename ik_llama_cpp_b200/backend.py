@@ -366,6 +366,45 @@ def moe_up_gate_merged(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, unar
     return dst
 
 
+def _batched_args(w: "QuantTensor | ExpertTensor", x_view: torch.Tensor, per_entry: bool):
+    """Shape and stride checks of mul_mat_batched (no device needed): (n_batch, n, col stride, batch stride) in floats."""
+    if x_view.dtype != torch.float32 or x_view.dim() != 3 or x_view.shape[2] != w.k:
+        raise ValueError(f"mul_mat_batched: x must be f32 [n_batch, n, K={w.k}], got {x_view.dtype} {tuple(x_view.shape)}")
+    n_batch, n, _ = x_view.shape
+    bs, cs, es = x_view.stride()
+    if es != 1 or min(n_batch, n) < 1 or (n > 1 and (cs % 4 or cs < w.k)) or (n_batch > 1 and (bs % 4 or bs < w.k)):
+        raise ValueError(f"mul_mat_batched: x rows must be contiguous with column / batch strides that are multiples of 4 floats and at least K apart, "
+                         f"got strides {tuple(x_view.stride())}")
+    cs, bs = (cs if n > 1 else w.k), (bs if n_batch > 1 else w.k)        # the stride of a dimension of size 1 is not used (torch may report any value)
+    if per_entry and not (isinstance(w, ExpertTensor) and w.n_expert == n_batch):
+        raise ValueError("mul_mat_batched: per_entry needs an ExpertTensor with one matrix per batch entry")
+    return n_batch, n, cs, bs
+
+
+def mul_mat_batched_workspace(w: "QuantTensor | ExpertTensor", n: int, n_batch: int, per_entry: bool, x_col_stride: int, x_batch_stride: int) -> int:
+    """Bytes of device workspace mul_mat_batched needs (b200q_mul_mat_batched_workspace; no device needed)."""
+    return int(_lib.lib().b200q_mul_mat_batched_workspace(w.ggml_type, w.m, w.k, n, n_batch, int(per_entry), x_col_stride, x_batch_stride))
+
+
+def mul_mat_batched(w: "QuantTensor | ExpertTensor", x_view: torch.Tensor, per_entry: bool, out: torch.Tensor | None = None) -> torch.Tensor:
+    """GGML_OP_MUL_MAT with a batch (ne[2] * ne[3] > 1) over a strided src1, in one launch sequence (b200q_mul_mat_batched).
+    x_view: f32 [n_batch, n, K], any view whose rows are contiguous (e.g. MLA's q_nope_perm, q.view(T, H, 192)[..., :128].transpose(0, 1));
+    per_entry: w is an ExpertTensor with one matrix per batch entry, else w (or matrix 0 of it) is broadcast over the batch.
+    -> dst f32 [n_batch, n, M], dst[b, j] = W_b . x_view[b, j]."""
+    n_batch, n, cs, bs = _batched_args(w, x_view, per_entry)
+    _require_cuda()
+    if not x_view.is_cuda:
+        raise ValueError("mul_mat_batched: x must be a CUDA tensor")
+    dst = out if out is not None else torch.empty((n_batch, n, w.m), dtype=torch.float32, device=x_view.device)
+    assert dst.shape == (n_batch, n, w.m) and dst.dtype == torch.float32 and dst.is_contiguous()
+    need = mul_mat_batched_workspace(w, n, n_batch, per_entry, cs, bs)
+    ws = _workspace(need, x_view.device) if need else None
+    with torch.cuda.device(x_view.device):
+        check(_lib.lib().b200q_mul_mat_batched(w.ggml_type, w.ptr, int(per_entry), x_view.data_ptr(), cs, bs, dst.data_ptr(), w.m, w.k, n, n_batch,
+                                               ws.data_ptr() if ws is not None else None, ws.numel() if ws is not None else 0, _stream()), "b200q_mul_mat_batched")
+    return dst
+
+
 def moe_combine(rows: torch.Tensor, weights: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
     """GGML_OP_MUL_MULTI_ADD (b200q_moe_combine): rows f32 [n_tokens, n_used, M], weights f32 [n_tokens, n_used] -> dst f32 [n_tokens, M],
     dst[t] = sum_u weights[t, u] * rows[t, u], summed in slot order in f32 as the reference CPU op."""

@@ -256,13 +256,24 @@ static bool b200_weight_ok(const ggml_tensor * w) {
     return w && b200_tensor_is_repacked(w) && w->buffer && b200_buffer_is_ours(w->buffer) && w->ne[3] == 1 &&
            w->ne[0] % ggml_blck_size(w->type) == 0 && w->ne[0] % 32 == 0 && b200q_plane_bytes(w->type, w->ne[1], w->ne[0]) > 0;
 }
-// MUL_MAT: w [K, M, E?] x [K, N, B2, B3] -> dst [M, N, B2, B3]; 2-D, or batched with w broadcast over the batch (ne02 == 1) or one weight matrix per
-// batch entry (ne02 == ne12, ne03 == 1)
+// Batched src1 [K, N, B2, B3] as b200q_mul_mat_batched takes it: f32 rows (nb[0] == 4) whose column and batch strides are multiples of 16 bytes, at
+// least one row apart, the B2 x B3 entries one stride apart (a permuted view such as MLA's q_nope_perm qualifies); strides returned in floats
+static bool b200_batched_x(const ggml_tensor * x, int64_t * col_stride, int64_t * batch_stride) {
+    if (x->nb[0] != sizeof(float) || (x->view_offs & 15)) return false;
+    const size_t row = x->ne[0] * sizeof(float), cs = x->nb[1], bs = x->ne[2] > 1 ? x->nb[2] : x->nb[3];
+    if (x->ne[2] > 1 && x->ne[3] > 1 && x->nb[3] != x->ne[2] * x->nb[2]) return false;
+    if ((cs & 15) || (bs & 15) || (x->ne[1] > 1 && cs < row) || bs < row) return false;
+    if (col_stride) *col_stride = (int64_t)(cs / sizeof(float));
+    if (batch_stride) *batch_stride = (int64_t)(bs / sizeof(float));
+    return true;
+}
+// MUL_MAT: w [K, M, E?] x [K, N, B2, B3] -> dst [M, N, B2, B3]; 2-D with a contiguous x, or batched (b200_batched_x) with w broadcast over the batch
+// (ne02 == 1) or one weight matrix per batch entry (ne02 == ne12, ne03 == 1)
 static bool b200_can_mul_mat(const ggml_tensor * w, const ggml_tensor * x, const ggml_tensor * dst) {
-    if (!b200_weight_ok(w) || !x || x->type != GGML_TYPE_F32 || !ggml_is_contiguous(x) || dst->type != GGML_TYPE_F32 || !ggml_is_contiguous(dst)) return false;
+    if (!b200_weight_ok(w) || !x || x->type != GGML_TYPE_F32 || dst->type != GGML_TYPE_F32 || !ggml_is_contiguous(dst)) return false;
     if (w->ne[0] != x->ne[0]) return false;
     if (!(w->ne[2] == 1 || (w->ne[2] == x->ne[2] && x->ne[3] == 1))) return false;
-    return true;
+    return x->ne[2] * x->ne[3] > 1 ? b200_batched_x(x, nullptr, nullptr) : ggml_is_contiguous(x);
 }
 // MoE expert ids: int32 [n_used, n_tokens], consecutive within a token.  The tokens' rows may lie further apart: ggml_top_k returns a view of the
 // argsort result (nb1 = n_expert * 4), and the scheduler's copy keeps that layout; graph_compute gathers such rows into its workspace.
@@ -320,14 +331,12 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
                 GGML_ASSERT(b200_can_mul_mat(w, x, node));
                 const int64_t m = w->ne[1], k = w->ne[0], n = x->ne[1];
                 const int64_t nbatch = x->ne[2] * x->ne[3];
-                if (nbatch > 1) {       // batched / broadcast MUL_MAT: one launch per batch entry (src0 broadcast over the batch or one matrix per entry)
-                    const size_t wstride = (size_t)b200q_plane_bytes(w->type, m, k);
-                    for (int64_t bi = 0; bi < nbatch; ++bi) {
-                        const char * W = (const char *)w->data + (w->ne[2] > 1 ? (size_t)bi * wstride : 0);
-                        const size_t need = b200q_mul_mat_workspace(w->type, m, k, n);
-                        void * ws = need ? c->workspace(need) : nullptr;
-                        B200Q_CHECK(b200q_mul_mat(w->type, W, (const float *)x->data + bi * n * k, (float *)node->data + bi * n * m, m, k, n, ws, need, c->stream));
-                    }
+                if (nbatch > 1) {       // batched / broadcast MUL_MAT over a strided src1 (src0 broadcast over the batch or one matrix per entry)
+                    int64_t cs = 0, bs = 0; b200_batched_x(x, &cs, &bs);
+                    const int per_entry = w->ne[2] > 1;
+                    const size_t need = b200q_mul_mat_batched_workspace(w->type, m, k, n, (int)nbatch, per_entry, cs, bs);
+                    void * ws = need ? c->workspace(need) : nullptr;
+                    B200Q_CHECK(b200q_mul_mat_batched(w->type, w->data, per_entry, (const float *)x->data, cs, bs, (float *)node->data, m, k, n, (int)nbatch, ws, need, c->stream));
                     break;
                 }
                 // q8_1 hand-off (n = 1): the previous node was the FUSED_UP_GATE that produced x and emitted its q8 image

@@ -78,7 +78,8 @@ def build_backend_plug(force: bool = False, verbose: bool = False) -> str | None
     return PLUG_LIB
 
 
-BACKEND_OPS_TESTS = ["test_mul_mat_backend", "test_moe_prefill_backend", "test_plug_graphs", "test_moe_merged_backend", "test_moe_combine_backend"]
+BACKEND_OPS_TESTS = ["test_mul_mat_backend", "test_moe_prefill_backend", "test_plug_graphs", "test_moe_merged_backend", "test_moe_combine_backend",
+                     "test_plug_mla"]
 
 
 def build_backend_ops_test(force: bool = False) -> str | None:

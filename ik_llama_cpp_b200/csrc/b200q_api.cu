@@ -380,9 +380,11 @@ static void moe_desc(b200q_mmvq_id_desc & d, int type, const moe_operands & o, i
     memset(&d, 0, sizeof d);
     d.type = type; d.W = o.W; d.W2 = o.W_gate; d.rows_layout = o.rows_layout; d.W_row0 = o.W_row0; d.W2_row0 = o.gate_row0;
     d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.act = unary; d.limit = limit;
+    d.x_tok_stride = (int64_t)nb1 * k; d.x_col_stride = k;      // MoE activations are contiguous; b200q_mul_mat_batched overrides both
 }
 static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst,
-                   int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream, const char * what) {
+                   int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream, const char * what,
+                   int64_t xs_tok = 0, int64_t xs_col = 0) {
     if (!o.W || !ids || !x || !dst || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
     dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
     if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "%s: activations must be 16-byte aligned", what);
@@ -396,7 +398,8 @@ static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t
     for (int t0 = 0; t0 < n_tokens; t0 += chunk) {
         const int nt = n_tokens - t0 < chunk ? n_tokens - t0 : chunk;
         b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
-        d.ids = ids + (int64_t)t0 * n_used; d.x = x + (int64_t)t0 * nb1 * k; d.dst = dst + (int64_t)t0 * n_used * m; d.n_tokens = nt;
+        if (xs_tok) { d.x_tok_stride = xs_tok; d.x_col_stride = xs_col; }
+        d.ids = ids + (int64_t)t0 * n_used; d.x = x + (int64_t)t0 * d.x_tok_stride; d.dst = dst + (int64_t)t0 * n_used * m; d.n_tokens = nt;
         d.sm_count = di.sm_count; d.pdl = opt_pdl();
         const int rc = check_launch(b200q_launch_mmvq_id(d, (cudaStream_t)stream), what);
         if (rc) return rc;
@@ -428,13 +431,15 @@ size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, in
     return moe_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate, m);
 }
 static int moe_gemm(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst, int64_t m, int64_t k,
-                    int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream, const char * what) {
+                    int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream, const char * what,
+                    int64_t xs_tok = 0, int64_t xs_col = 0) {
     if (!o.W || !ids || !x || !dst || !workspace || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
     dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
     if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
     if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, o.W_gate != nullptr))
         return fail(B200Q_E_SHAPE, "%s: shape not supported by the grouped GEMM (K %% 256, n_expert <= 1024, type)", what);
     b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
+    if (xs_tok) { d.x_tok_stride = xs_tok; d.x_col_stride = xs_col; }
     d.ids = ids; d.x = x; d.dst = dst; d.n_tokens = n_tokens; d.sm_count = di.sm_count;
     return check_launch(b200q_launch_moe_gemm(d, workspace, workspace_bytes, (cudaStream_t)stream), what);
 }
@@ -478,6 +483,106 @@ int b200q_moe_combine(const float * rows, const float * weights, float * dst, in
     if ((d0 < r1 && r0 < d1) || (d0 < w1 && w0 < d1)) return fail(B200Q_E_ARG, "%s: dst overlaps an input", what);
     return check_launch(b200q_launch_moe_combine(rows, weights, dst, m, n_used, n_tokens, (cudaStream_t)stream), what);
 }
+/* Batched MUL_MAT as MUL_MAT_ID with identity routing: token := batch entry, slot := column, n_used = nb1 = n, ids[b][j] = b (per entry,
+ * n_expert = n_batch) or 0 (broadcast, n_expert = 1), written into the workspace by k_batch_ids.  With identity routing every entry gets exactly n
+ * rows, so the MoE crossover (routed slots) does not apply.  Cut points from scripts/bench_batched.py on DeepSeek-V3's MLA products, 128 and 16
+ * heads, Q8_0 and IQ4_NL, n = 1 ... 512, on an H100 80GB HBM3 at 700 W (DESIGN.md §4):
+ *  - the grouped GEMM, where it is eligible (K % 256), from 128 slots (n_batch * n) on: wv_b at 16 heads is 1.3x slower than the mat-vec at 64
+ *    slots and 1.3x faster at 128; a type without a fused GEMM kernel (Q8_0) dequantises every entry's matrix first, so with one column per entry
+ *    (128 heads, n = 1: 33 us against 26 us) the mat-vec stays faster;
+ *  - otherwise the identity-routed mat-vec up to 16 columns per entry (wk_b at 128 heads: 580 us against 904 us for one GEMM per head at n = 16,
+ *    1184 us against 957 us at n = 32), one dense GEMM per entry above.  It beats one dense mat-vec per entry at every n <= 8 (wk_b at 128 heads:
+ *    41 us against 428 us at n = 1, 291 us against 371 us at n = 8). */
+enum batched_path { BATCHED_ONE = 0, BATCHED_VEC, BATCHED_ENTRY_VEC, BATCHED_GROUPED, BATCHED_DENSE };
+static constexpr int64_t BATCHED_GROUPED_MIN_SLOTS = 128;
+static constexpr int64_t BATCHED_VEC_MAX_N = 16;
+struct batched_plan { int path; int64_t n_cols, x_stride; int n_expert; size_t ids_bytes, ws_bytes; };
+// argument / shape checks of the batched entry and its plan; returns a B200Q_E_* code (the failure text is set) or 0
+static int plan_batched(int type, int64_t m, int64_t k, int64_t n, int n_batch, int per_entry, int64_t cs, int64_t bs, batched_plan & p, const char * what) {
+    p = batched_plan{};
+    if (m < 1 || k < 1 || n < 1 || n_batch < 1 || (per_entry != 0 && per_entry != 1)) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    if (cs < 0 || bs < 0 || (cs & 3) || (bs & 3) || (n > 1 && cs < k) || (n_batch > 1 && bs < k))
+        return fail(B200Q_E_ARG, "%s: strides must be multiples of 4 floats, at least k where they are used", what);
+    if (n > INT32_MAX || n * n_batch > INT32_MAX) return fail(B200Q_E_SHAPE, "%s: too many columns", what);
+    b200q_layout L; if (const int rc = b200q_make_layout(type, m, k, &L)) return check_launch(rc, what);
+    const int64_t max_cols = b200q_mmvq_max_cols(k);
+    // one matrix over columns a constant stride apart (broadcast with x_batch_stride == n * x_col_stride, or one entry): a plain 2-D product, as long
+    // as it stays on the side of the mat-vec / GEMM cut (n <= 8) each entry would take on its own
+    const bool uniform = (!per_entry || n_batch == 1) && (n == 1 || n_batch == 1 || bs == n * cs);
+    if (uniform && (n * n_batch <= 8 || n > 8)) {
+        p.path = BATCHED_ONE; p.n_cols = n * n_batch; p.x_stride = n == 1 ? (n_batch > 1 ? bs : k) : cs;
+        if (p.n_cols <= 8) { if (max_cols < 1) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)k); }
+        else p.ws_bytes = b200q_gemm_workspace_bytes(type, m, k, p.n_cols);
+        return 0;
+    }
+    // a broadcast matrix with up to 8 columns per entry: the dense mat-vec of each entry (it reads the matrix once per entry for all its columns)
+    if (!per_entry && n <= 8) {
+        if (max_cols < n) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)k);
+        p.path = BATCHED_ENTRY_VEC;
+        return 0;
+    }
+    p.n_expert = per_entry ? n_batch : 1;
+    p.ids_bytes = (size_t)b200q_align_up(n * n_batch * 4, 256);
+    const bool grouped = b200q_moe_gemm_shape_ok(type, m, k, (int)n, (int)n, n_batch, p.n_expert, 0) && n * n_batch >= BATCHED_GROUPED_MIN_SLOTS &&
+                         (n > 1 || b200q_gemm_fused_type(type));
+    if (grouped) {
+        p.path = BATCHED_GROUPED; p.ws_bytes = p.ids_bytes + b200q_moe_gemm_workspace_bytes(type, m, k, n * n_batch, p.n_expert, 0, m);
+    } else if (n <= BATCHED_VEC_MAX_N && max_cols >= n) {
+        p.path = BATCHED_VEC; p.ws_bytes = p.ids_bytes;
+    } else if (n <= 8) {
+        return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)k);
+    } else {
+        p.path = BATCHED_DENSE; p.ids_bytes = 0; p.ws_bytes = b200q_gemm_workspace_bytes(type, m, k, n);
+    }
+    return 0;
+}
+size_t b200q_mul_mat_batched_workspace(int type, int64_t m, int64_t k, int64_t n, int n_batch, int per_entry, int64_t x_col_stride, int64_t x_batch_stride) {
+    batched_plan p;
+    return plan_batched(type, m, k, n, n_batch, per_entry, x_col_stride, x_batch_stride, p, "b200q_mul_mat_batched_workspace") ? 0 : p.ws_bytes;
+}
+int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float * x, int64_t x_col_stride, int64_t x_batch_stride,
+                          float * dst, int64_t m, int64_t k, int64_t n, int n_batch, void * workspace, size_t workspace_bytes, void * stream) {
+    static const char * what = "b200q_mul_mat_batched";
+    if (!W || !x || !dst || ((uintptr_t)x & 15) || ((uintptr_t)workspace & 255)) return fail(B200Q_E_ARG, "%s: bad argument (x 16-byte, workspace 256-byte aligned)", what);
+    batched_plan p;
+    if (const int rc = plan_batched(type, m, k, n, n_batch, per_entry, x_col_stride, x_batch_stride, p, what)) return rc;
+    if (workspace_bytes < p.ws_bytes || (p.ws_bytes && !workspace)) return fail(B200Q_E_NOMEM, "%s: workspace too small", what);
+    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p.path == BATCHED_ONE) {
+        if (p.n_cols <= 8) {
+            b200q_mmvq_desc d; memset(&d, 0, sizeof d);
+            d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst, nullptr, m}; d.K = k; d.x = x; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+            return mmvq_cols(d, (int)p.n_cols, p.x_stride, st, what);
+        }
+        return check_launch(b200q_launch_gemm(type, W, x, p.x_stride, dst, m, k, p.n_cols, workspace, workspace_bytes, di.sm_count, opt_fused(), st), what);
+    }
+    if (p.path == BATCHED_ENTRY_VEC) {  // the broadcast matrix, one dense mat-vec per entry over its strided columns
+        for (int b = 0; b < n_batch; ++b) {
+            b200q_mmvq_desc d; memset(&d, 0, sizeof d);
+            d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst + (int64_t)b * n * m, nullptr, m}; d.K = k; d.x = x + b * x_batch_stride;
+            d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+            if (const int rc = mmvq_cols(d, (int)n, x_col_stride, st, what)) return rc;
+        }
+        return B200Q_OK;
+    }
+    if (p.path == BATCHED_DENSE) {      // one GEMM per entry over its strided columns, on one workspace (stream-ordered reuse)
+        const int64_t wstride = per_entry ? b200q_plane_bytes(type, m, k) : 0;
+        for (int b = 0; b < n_batch; ++b) {
+            const int rc = check_launch(b200q_launch_gemm(type, (const char *)W + b * wstride, x + b * x_batch_stride, x_col_stride, dst + (int64_t)b * n * m, m, k, n,
+                                                          workspace, workspace_bytes, di.sm_count, opt_fused(), st), what);
+            if (rc) return rc;
+        }
+        return B200Q_OK;
+    }
+    int32_t * ids = (int32_t *)workspace;
+    if (const int rc = check_launch(b200q_launch_batch_ids(ids, n_batch, (int)n, per_entry, st), what)) return rc;
+    const moe_operands o{W, nullptr, m, 0, 0};
+    if (p.path == BATCHED_VEC) return moe_vec(type, o, p.n_expert, ids, x, dst, m, k, (int)n, (int)n, n_batch, 0, 0.0f, stream, what, x_batch_stride, x_col_stride);
+    return moe_gemm(type, o, p.n_expert, ids, x, dst, m, k, (int)n, (int)n, n_batch, 0, 0.0f, (char *)workspace + p.ids_bytes, workspace_bytes - p.ids_bytes, stream, what,
+                    x_batch_stride, x_col_stride);
+}
+
 int b200q_mul_mat_host(int type, const void * W, const float * x_host, float * dst_host, int64_t m, int64_t k, int64_t n, void * stream) {
     cudaStream_t st = (cudaStream_t)stream; cudaError_t e; int rc;
     const size_t xb = (size_t)n * k * sizeof(float), yb = (size_t)n * m * sizeof(float), wsb = b200q_mul_mat_workspace(type, m, k, n);

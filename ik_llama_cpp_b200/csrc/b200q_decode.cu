@@ -388,7 +388,7 @@ int b200q_launch_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
     mmvq_id_args a; memset(&a, 0, sizeof a);
     a.P = b200q_planes_at((const uint8_t *)d.W, L, d.W_row0); if (d.W2) a.P2 = b200q_planes_at((const uint8_t *)d.W2, L, d.W2_row0);
     a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used; a.n_used = d.n_used; a.nb1 = d.nb1; a.ncx = d.n_tokens * d.nb1;
-    a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit;
+    a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit; a.xs_tok = d.x_tok_stride; a.xs_col = d.x_col_stride;
     b200q_mmvq_plan p; if (const int prc = b200q_plan_mmvq_id(d, p)) return prc;
     const void * k = nullptr;
     switch (d.type) {

@@ -191,6 +191,7 @@ struct mmvq_id_args {
     const int32_t * ids;            // [n_slots] expert per slot
     int n_expert, n_slots, n_used, nb1, ncx;   // slots = n_tokens * n_used; x columns = n_tokens * nb1, column of slot s = (s / n_used) * nb1 + (s % n_used) % nb1
     int64_t M, K; const float * x; float * dst; int act; float limit;
+    int64_t xs_tok, xs_col;         // column c = t * nb1 + j starts at x + t * xs_tok + j * xs_col
 };
 template <int TYPE, bool UPGATE>
 __global__ void __launch_bounds__(512, 1) k_mmvq_id(const mmvq_id_args a) {
@@ -202,7 +203,12 @@ __global__ void __launch_bounds__(512, 1) k_mmvq_id(const mmvq_id_args a) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     pdl_trigger();
     pdl_wait();
-    for (int c = 0; c < a.ncx; ++c) quantize_x_to_smem<1>(a.x + (int64_t)c * K, K, K, sq + (size_t)c * K, sd + c * n32, sis + c * n32, threadIdx.x, blockDim.x);
+    // the columns are quantised concurrently, each by a group of whole warps with a thread per 8 floats (the whole CTA once K >= 8 x blockDim)
+    const int gs = min((int)blockDim.x, (int)((K / 8 + 31) / 32 * 32)), ng = blockDim.x / gs, grp = threadIdx.x / gs;
+    if (grp < ng)
+        for (int c = grp; c < a.ncx; c += ng)
+            quantize_x_to_smem<1>(a.x + (int64_t)(c / a.nb1) * a.xs_tok + (int64_t)(c % a.nb1) * a.xs_col, K, K, sq + (size_t)c * K, sd + c * n32,
+                                  sis + c * n32, threadIdx.x - grp * gs, gs);
     __shared__ uint32_t kv_slot[128];
     const b200q_kv4 T = b200q_kv4_init_via_smem(kv_slot);     // includes the __syncthreads() that publishes the activations
     constexpr int U = UPGATE ? 2 : 4;

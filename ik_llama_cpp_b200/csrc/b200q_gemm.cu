@@ -603,10 +603,11 @@ __global__ void k_mul_unary(const float * gate /* may alias dst: no __restrict__
 
 // f32 [N][K] (row stride xs) -> bf16 [N][K].  HBM-bound glue between the GEMMs (12 MB per 512 x 4096 activation): a thread converts 8 consecutive
 // values (two LDG.128 -> one STG.128) and keeps U such groups in flight, so that enough loads are outstanding to approach HBM bandwidth.
-// MAP (MoE gather): output row n reads input row row_map[n]; a negative entry (past the routed rows) gives a zero row.
+// MAP (MoE gather): output row n reads activation column c = row_map[n] = t * nb1 + j, at x + t * xs + j * xs_col; a negative entry (past the
+// routed rows) gives a zero row.
 template <bool MAP = false>
 __global__ void __launch_bounds__(256) k_f32_to_bf16(const float * __restrict__ x, int64_t xs, __nv_bfloat16 * __restrict__ out, int64_t K, int64_t N,
-                                                     const int * __restrict__ row_map = nullptr) {
+                                                     const int * __restrict__ row_map = nullptr, int nb1 = 1, int64_t xs_col = 0) {
     constexpr int U = 4;
     const int64_t k8 = K / 8, total8 = N * k8, stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < total8; i0 += U * stride) {
@@ -618,7 +619,8 @@ __global__ void __launch_bounds__(256) k_f32_to_bf16(const float * __restrict__ 
                 const int64_t n = i / k8, c = i % k8;
                 const int64_t src = MAP ? (int64_t)__ldg(row_map + n) : n;
                 if (MAP && src < 0) { a[u] = b[u] = make_float4(0.f, 0.f, 0.f, 0.f); continue; }
-                const float4 * p = reinterpret_cast<const float4 *>(x + src * xs + 8 * c); a[u] = __ldg(p); b[u] = __ldg(p + 1);
+                const int64_t off = MAP ? (src / nb1) * xs + (src % nb1) * xs_col : src * xs;
+                const float4 * p = reinterpret_cast<const float4 *>(x + off + 8 * c); a[u] = __ldg(p); b[u] = __ldg(p + 1);
             }
         }
 #pragma unroll
@@ -881,11 +883,12 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
 
 int b200q_gemm_fused_type(int type) { return gemmq_supported(type) ? 1 : 0; }
 
-// MoE gather: bf16 [N][K] whose row n is row row_map[n] of x (rows K floats apart); a negative entry gives a zero row
-int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, void * out, int64_t K, int64_t N, cudaStream_t st) {
-    if (K % 8 || ((uintptr_t)x & 15) || ((uintptr_t)out & 15)) return -2;
+// MoE gather: bf16 [N][K] whose row n is activation column row_map[n] of x (see b200q_internal.h); a negative entry gives a zero row
+int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, int nb1, int64_t x_tok_stride, int64_t x_col_stride, void * out, int64_t K, int64_t N,
+                                  cudaStream_t st) {
+    if (K % 8 || nb1 < 1 || (x_tok_stride | x_col_stride) & 3 || ((uintptr_t)x & 15) || ((uintptr_t)out & 15)) return -2;
     const int64_t total8 = N * (K / 8); int64_t nb = (total8 + 256 * 4 - 1) / (256 * 4); if (nb > 132 * 8) nb = 132 * 8; if (nb < 1) nb = 1;
-    k_f32_to_bf16<true><<<(unsigned)nb, 256, 0, st>>>(x, K, (__nv_bfloat16 *)out, K, N, row_map);
+    k_f32_to_bf16<true><<<(unsigned)nb, 256, 0, st>>>(x, x_tok_stride, (__nv_bfloat16 *)out, K, N, row_map, nb1, x_col_stride);
     return (int)cudaGetLastError();
 }
 

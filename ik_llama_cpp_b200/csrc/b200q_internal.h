@@ -72,12 +72,14 @@ static inline size_t b200q_q8_image_bytes(int64_t k) { return (size_t)(k + 12 * 
 int b200q_launch_repack(const void * wire, void * planes, const b200q_layout & L, int inverse, cudaStream_t st);
 int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out, cudaStream_t st);
 // MoE decode: W = n_expert matrices [rows_layout x K], b200q_plane_bytes(type, rows_layout, K) apart; ids device int32 [n_tokens][n_used];
-// x f32 [n_tokens][nb1][K]; dst f32 [n_tokens][n_used][M].  An operand is rows [row0, row0 + M) of its expert matrices: the split form is
+// x f32 [n_tokens][nb1][K]: column (t, j) starts at x + t * x_tok_stride + j * x_col_stride (floats; the MoE ops pass the contiguous nb1 * K, K);
+// dst f32 [n_tokens][n_used][M].  An operand is rows [row0, row0 + M) of its expert matrices: the split form is
 // W_row0 = W2_row0 = 0 with rows_layout = M, merged up/gate experts ([gate; up], rows_layout = 2 M) are W = W2 with W_row0 = M (up), W2_row0 = 0 (gate).
 struct b200q_mmvq_id_desc {
     int type; const void * W; const void * W2; const int32_t * ids; const float * x; float * dst;
     int64_t M, K; int n_expert, n_used, nb1, n_tokens; int act; float limit; int sm_count; int pdl;
     int64_t rows_layout, W_row0, W2_row0;
+    int64_t x_tok_stride, x_col_stride;
 };
 int b200q_launch_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
 int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
@@ -115,7 +117,11 @@ struct b200q_moe_gemm {
     const void * xb; int bn;                                   // bf16 [n_rows][K] in expert-sorted order; tile width (128 / 256)
     b200q_moe_route rt;
 };
-int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, void * out, int64_t K, int64_t N, cudaStream_t st);
+// MoE gather: row n of out is activation column row_map[n] = t * nb1 + j of x, at x + t * x_tok_stride + j * x_col_stride
+int b200q_launch_f32_to_bf16_rows(const float * x, const int * row_map, int nb1, int64_t x_tok_stride, int64_t x_col_stride, void * out, int64_t K, int64_t N,
+                                  cudaStream_t st);
+// ids [n_batch][n] of a batched MUL_MAT run as MUL_MAT_ID: the batch entry b (per_entry) or 0 (one matrix broadcast over the batch)
+int b200q_launch_batch_ids(int32_t * ids, int n_batch, int n, int per_entry, cudaStream_t st);
 int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t ws_bytes, cudaStream_t st);
 // dequantise experts e0 .. e0+n_e-1 of an expert tensor (L: one expert; experts L.total_bytes apart) into bf16 [n_e][M][K]; with bounds, the experts
 // that received no rows are skipped

@@ -110,7 +110,18 @@ k_moe_combine(const T * __restrict__ rows, const float * __restrict__ w, T * __r
     }
 }
 
+__global__ void k_batch_ids(int32_t * __restrict__ ids, int n, int64_t total, int per_entry) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) ids[i] = per_entry ? (int32_t)(i / n) : 0;
+}
+
 }  // namespace
+
+int b200q_launch_batch_ids(int32_t * ids, int n_batch, int n, int per_entry, cudaStream_t st) {
+    const int64_t total = (int64_t)n_batch * n;
+    const int64_t g = std::min<int64_t>((total + 255) / 256, 132 * 4);
+    k_batch_ids<<<(unsigned)g, 256, 0, st>>>(ids, n, total, per_entry);
+    return (int)cudaGetLastError();
+}
 
 int b200q_launch_moe_combine(const float * rows, const float * w, float * dst, int64_t m, int n_used, int n_tokens, cudaStream_t st) {
     const bool v4 = m % 4 == 0 && !((uintptr_t)rows & 15) && !((uintptr_t)dst & 15);
@@ -148,7 +159,7 @@ int b200q_launch_moe_gemm(const b200q_mmvq_id_desc & d, void * ws, size_t ws_byt
     const int bn = moe_tile_rows(n_slots, d.n_expert);
     k_moe_route<<<1, ROUTE_THREADS, 0, st>>>(d.ids, (int)n_slots, d.n_used, d.nb1, d.n_expert, bn, bounds, tile_start, tiles, slot, col, d.dst, up, d.M);
     int rc = (int)cudaGetLastError(); if (rc) return rc;
-    if ((rc = b200q_launch_f32_to_bf16_rows(d.x, col, b + L.xb, d.K, n_slots, st))) return rc;
+    if ((rc = b200q_launch_f32_to_bf16_rows(d.x, col, d.nb1, d.x_tok_stride, d.x_col_stride, b + L.xb, d.K, n_slots, st))) return rc;
     b200q_moe_gemm g{};
     g.type = d.type; g.n_seg = ug ? 2 : 1; g.W[0] = d.W; g.dst[0] = ug ? up : d.dst; g.W[1] = d.W2; g.dst[1] = d.dst;
     g.row0[0] = d.W_row0; g.row0[1] = d.W2_row0; g.rows_layout = d.rows_layout;

@@ -111,6 +111,7 @@ const void * wire_mmvq_kernel(const b200q_mmvq_plan & p) {
 struct wire_id_args {
     const uint8_t * W; const uint8_t * W2; int64_t estride; const int32_t * ids; int n_expert, n_slots, n_used, nb1, ncx;
     int64_t M, K; const float * x; float * dst; int act; float limit;
+    int64_t xs_tok, xs_col;
 };
 template <int TYPE, bool UPGATE>
 __global__ void __launch_bounds__(256) k_wire_mmvq_id(const wire_id_args a) {
@@ -122,7 +123,12 @@ __global__ void __launch_bounds__(256) k_wire_mmvq_id(const wire_id_args a) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     pdl_trigger();
     pdl_wait();
-    for (int c = 0; c < a.ncx; ++c) quantize_x_to_smem<1>(a.x + (int64_t)c * K, K, K, sq + (size_t)c * K, sd + c * n32, sis + c * n32, threadIdx.x, blockDim.x);
+    // the columns are quantised concurrently, each by a group of whole warps with a thread per 8 floats (the whole CTA once K >= 8 x blockDim)
+    const int gs = min((int)blockDim.x, (int)((K / 8 + 31) / 32 * 32)), ng = blockDim.x / gs, grp = threadIdx.x / gs;
+    if (grp < ng)
+        for (int c = grp; c < a.ncx; c += ng)
+            quantize_x_to_smem<1>(a.x + (int64_t)(c / a.nb1) * a.xs_tok + (int64_t)(c % a.nb1) * a.xs_col, K, K, sq + (size_t)c * K, sd + c * n32,
+                                  sis + c * n32, threadIdx.x - grp * gs, gs);
     __syncthreads();
     const int64_t total = (int64_t)a.n_slots * a.M;
     for (int64_t g = (int64_t)blockIdx.x * nwarps + warp; g < total; g += (int64_t)gridDim.x * nwarps) {
@@ -163,6 +169,7 @@ int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st) {
     a.W = (const uint8_t *)d.W + b200q_row_offset(L, 0, d.W_row0); a.W2 = d.W2 ? (const uint8_t *)d.W2 + b200q_row_offset(L, 0, d.W2_row0) : nullptr;
     a.estride = L.total_bytes; a.ids = d.ids; a.n_expert = d.n_expert; a.n_slots = d.n_tokens * d.n_used;
     a.n_used = d.n_used; a.nb1 = d.nb1; a.ncx = d.n_tokens * d.nb1; a.M = d.M; a.K = d.K; a.x = d.x; a.dst = d.dst; a.act = d.act; a.limit = d.limit;
+    a.xs_tok = d.x_tok_stride; a.xs_col = d.x_col_stride;
     b200q_mmvq_plan p; if (const int prc = b200q_plan_mmvq_id(d, p)) return prc;
     const void * k = nullptr;
     switch (d.type) {

@@ -216,6 +216,24 @@ B200Q_API int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_e
  * range need no care: MUL_MAT_ID gives them zero rows.  All pointers 4-byte aligned; dst must not overlap rows or weights (B200Q_E_ARG).
  * Writes only dst; no workspace, allocation or synchronisation (capturable). */
 B200Q_API int b200q_moe_combine(const float * rows, const float * weights, float * dst, int64_t m, int n_used, int n_tokens, void * stream);
+/* ---- batched MUL_MAT: GGML_OP_MUL_MAT with ne[2] * ne[3] > 1, over strided activations, in one launch sequence ----
+ * (the per-head products of absorbed MLA, q_nope2 = wk_b x q_nope_perm and kqv = wv_b x kqv_compressed_perm, src/graphs/build_deepseek2.cpp:1030-1036,
+ * 1145-1162; the weights are Q8_0 [k, m, n_head] made by llm_prepare_mla, src/llama.cpp:3014, 3054)
+ *     dst[b][j][i] = W_b[i] . x[b * x_batch_stride + j * x_col_stride + 0 .. k)      b < n_batch, j < n, i < m
+ * W_b = W (per_entry = 0: one matrix broadcast over the batch) or W + b * b200q_plane_bytes(type, m, k) (per_entry = 1: n_batch matrices, each uploaded
+ * with b200q_set_tensor); strides in floats; dst f32 contiguous [n_batch][n][m] (ggml's dst of a batched MUL_MAT).
+ * Conditions: x 16-byte aligned; both strides non-negative multiples of 4 floats, x_col_stride >= k when n > 1 and x_batch_stride >= k when n_batch > 1
+ * (otherwise B200Q_E_ARG); k a multiple of the type's block and n * n_batch <= INT32_MAX (otherwise B200Q_E_SHAPE); workspace 256-byte aligned.
+ * It runs the MoE kernels with identity routing (ids[b][j] = b, or 0 when broadcast, written into the workspace): the grouped MoE GEMM where it is
+ * eligible (k % 256 == 0, n_batch <= 1024) from 128 slots (n_batch * n) on, for types without a fused GEMM kernel only from n = 2 on; otherwise the
+ * MoE mat-vec kernel up to n = 16 (one launch, or entry chunks when the n_batch * n quantised columns exceed shared memory), one GEMM per entry
+ * above.  A broadcast W over columns a constant stride apart is one 2-D product.
+ * b200q_mul_mat_batched_workspace: the bytes the call needs (0 for a 2-D product with n * n_batch <= 8, and for any rejected argument); needs no device.
+ * No host round trip, allocation or synchronisation: the call can be captured in a CUDA graph. */
+B200Q_API size_t b200q_mul_mat_batched_workspace(int type, int64_t m, int64_t k, int64_t n, int n_batch, int per_entry,
+                                                 int64_t x_col_stride, int64_t x_batch_stride);
+B200Q_API int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float * x, int64_t x_col_stride, int64_t x_batch_stride,
+                                    float * dst, int64_t m, int64_t k, int64_t n, int n_batch, void * workspace, size_t workspace_bytes, void * stream);
 /* same through HOST activations/results: H2D(x) -> mul_mat -> D2H(dst), synchronous (end-to-end entry point) */
 B200Q_API int b200q_mul_mat_host(int type, const void * W_planes_dev, const float * x_host, float * dst_host,
                        int64_t m, int64_t k, int64_t n, void * stream);

@@ -84,6 +84,9 @@ def lib() -> ctypes.CDLL:
         L.b200q_mul_mat_id_workspace.argtypes = [i32, i64, i64, i32, i32, i32, i32, i32]
         L.b200q_mul_mat_id_gemm.argtypes = [i32, vp, vp, i32, vp, vp, vp, i64, i64, i32, i32, i32, i32, c_float, vp, c_size_t, vp]
         L.b200q_mul_mat_id.argtypes = [i32, vp, vp, i32, vp, vp, vp, i64, i64, i32, i32, i32, i32, c_float, vp, c_size_t, vp]
+    if hasattr(L, "b200q_mul_mat_id_gemm_workspace"):
+        L.b200q_mul_mat_id_gemm_workspace.restype = c_size_t
+        L.b200q_mul_mat_id_gemm_workspace.argtypes = [i32, i64, i64, i32, i32, i32, i32, i32]
     if hasattr(L, "b200q_moe_up_gate_merged"):
         L.b200q_moe_up_gate_merged_workspace.restype = c_size_t
         L.b200q_moe_up_gate_merged_workspace.argtypes = [i32, i64, i64, i32, i32, i32, i32]

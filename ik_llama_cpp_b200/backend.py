@@ -164,8 +164,7 @@ def mul_mat(w: QuantTensor, x: torch.Tensor, out: torch.Tensor | None = None, x_
             check(L.b200q_mul_mat_vec_q8(w.ggml_type, w.ptr, x.data_ptr(), q8_in.buf.data_ptr(), dst.data_ptr(), w.m, w.k, bp, _stream()), "b200q_mul_mat_vec_q8")
         elif n > MMVQ_MAX_BATCH_SIZE and x_bf16 is not None:
             assert x_bf16.dtype == torch.bfloat16 and x_bf16.shape == x.shape and x_bf16.is_contiguous()
-            need = w.m * w.k * 2 + 256
-            ws = _workspace(need, x.device)
+            ws = _workspace(L.b200q_mul_mat_workspace(w.ggml_type, w.m, w.k, n), x.device)
             check(L.b200q_mul_mat_gemm_bf16(w.ggml_type, w.ptr, x_bf16.data_ptr(), dst.data_ptr(), w.m, w.k, n, ws.data_ptr(), ws.numel(), _stream()), "b200q_mul_mat_gemm_bf16")
         elif n <= MMVQ_MAX_BATCH_SIZE:
             check(L.b200q_mul_mat_vec(w.ggml_type, w.ptr, x.data_ptr(), dst.data_ptr(), w.m, w.k, n, x.stride(0), bp, _stream()), "b200q_mul_mat_vec")
@@ -195,7 +194,7 @@ def mul_mat_multi(ws: list[QuantTensor], x: torch.Tensor, outs: list[torch.Tenso
             check(L.b200q_mul_mat_vec_multi(ws[0].ggml_type, nt, Wp, Dp, Mp, ws[0].k, x.data_ptr(), n, x.stride(0), _stream()), "b200q_mul_mat_vec_multi")
         elif x_bf16 is not None:
             assert x_bf16.dtype == torch.bfloat16 and x_bf16.shape == x.shape and x_bf16.is_contiguous()
-            wsb = _workspace(max(w.m for w in ws) * ws[0].k * 2 + 256, x.device)
+            wsb = _workspace(L.b200q_mul_mat_multi_workspace(ws[0].ggml_type, nt, Mp, ws[0].k, n), x.device)
             check(L.b200q_mul_mat_gemm_multi_bf16(ws[0].ggml_type, nt, Wp, Dp, Mp, ws[0].k, x_bf16.data_ptr(), n, wsb.data_ptr(), wsb.numel(), _stream()),
                   "b200q_mul_mat_gemm_multi_bf16")
         else:
@@ -234,8 +233,7 @@ def fused_up_gate(up: QuantTensor, gate: QuantTensor, x: torch.Tensor, unary: st
             assert xb.dtype == torch.bfloat16 and xb.shape == x.shape and xb.is_contiguous()
             if out_bf16 is not None:
                 assert out_bf16.dtype == torch.bfloat16 and out_bf16.shape == dst.shape and out_bf16.is_contiguous()
-            need = (up.m * n * 4 + 255) // 256 * 256 + up.m * up.k * 2 + 256
-            ws = _workspace(need, x.device)
+            ws = _workspace(L.b200q_fused_up_gate_workspace(up.ggml_type, up.m, up.k, n), x.device)
             check(L.b200q_fused_up_gate_gemm_bf16(up.ggml_type, up.ptr, gate.ptr, xb.data_ptr(), dst.data_ptr(),
                                                   out_bf16.data_ptr() if out_bf16 is not None else None, up.m, up.k, n,
                                                   UNARY[unary], float(limit), ws.data_ptr(), ws.numel(), _stream()), "b200q_fused_up_gate_gemm_bf16")
@@ -314,8 +312,7 @@ def mul_mat_id_gemm(w: ExpertTensor, x: torch.Tensor, ids: torch.Tensor, gate: "
     n_tokens, nb1, n_used = _mul_mat_id_args(w, x, ids, gate)
     dst = out if out is not None else torch.empty((n_tokens, n_used, w.m), dtype=torch.float32, device=x.device)
     L = _lib.lib()
-    # the workspace query returns 0 below the dispatch threshold: size it from a batch above it (the layout only grows with the batch)
-    need = mul_mat_id_workspace(w, max(n_tokens, 8 * w.n_expert // n_used + 1), n_used, nb1, gate is not None)
+    need = L.b200q_mul_mat_id_gemm_workspace(w.ggml_type, w.m, w.k, n_used, nb1, n_tokens, w.n_expert, int(gate is not None))
     ws = _workspace(need, x.device)
     with torch.cuda.device(x.device):
         check(L.b200q_mul_mat_id_gemm(w.ggml_type, w.ptr, gate.ptr if gate is not None else None, w.n_expert, ids.data_ptr(), x.data_ptr(), dst.data_ptr(),

@@ -35,6 +35,11 @@ dev_info & device_info() {
     }
     return info[dev];
 }
+// the SM count of the current device; without a device, B200Q_E_CUDA
+int device_sms(int & sms, const char * what) {
+    const dev_info & di = device_info(); sms = di.sm_count;
+    return di.ok ? B200Q_OK : fail(B200Q_E_CUDA, "%s: no CUDA device", what);
+}
 int check_launch(int rc, const char * what) {
     if (rc == 0) return B200Q_OK;
     if (rc == -1) return fail(B200Q_E_TYPE, "%s: unsupported ggml type", what);
@@ -129,18 +134,26 @@ int b200q_get_tensor(int type, const void * planes_dev, void * wire_host, int64_
 static thread_local b200q_mmvq_desc g_next; static thread_local bool g_next_valid = false;
 static inline void attach_next(b200q_mmvq_desc & d) { d.next = nullptr; if (g_next_valid && opt_pf()) d.next = &g_next; g_next_valid = false; }
 
+// a decode launch's descriptor, zeroed, with type, K, x and the launch options; the caller adds its segments and its own fields
+static int mmvq_desc(b200q_mmvq_desc & d, int type, int64_t k, const float * x, const char * what) {
+    int sms = 0; if (const int rc = device_sms(sms, what)) return rc;
+    memset(&d, 0, sizeof d);
+    d.type = type; d.K = k; d.x = x; d.sm_count = sms; d.pdl = opt_pdl(); d.ring = opt_ring();
+    return B200Q_OK;
+}
+
 int b200q_decode_prefetch_next(int type, int n_tensors, const void * const * W, const void * W_gate, const int64_t * m, int64_t k) {
     g_next_valid = false;
     if (n_tensors < 1 || n_tensors > B200Q_MAX_SEGS || !W || !m || (W_gate && n_tensors != 1)) return fail(B200Q_E_ARG, "b200q_decode_prefetch_next: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_decode_prefetch_next: no CUDA device");
-    memset(&g_next, 0, sizeof g_next);
-    g_next.type = type; g_next.n_seg = n_tensors; g_next.K = k; g_next.ncols = 1; g_next.sm_count = di.sm_count; g_next.ring = opt_ring();
+    if (const int rc = mmvq_desc(g_next, type, k, nullptr, "b200q_decode_prefetch_next")) return rc;
+    g_next.n_seg = n_tensors; g_next.ncols = 1;
     for (int i = 0; i < n_tensors; ++i) g_next.seg[i] = {W[i], i == 0 ? W_gate : nullptr, nullptr, nullptr, m[i]};
     g_next_valid = true;
     return B200Q_OK;
 }
 
-static int mmvq_cols(b200q_mmvq_desc & d, int n, int64_t x_stride, cudaStream_t st, const char * what) {
+// every decode entry but the tensor-parallel one launches here: n columns x_stride floats apart (0: K); `plan`: what the last piece launched
+static int mmvq_cols(b200q_mmvq_desc & d, int n, int64_t x_stride, cudaStream_t st, const char * what, b200q_mmvq_plan * plan = nullptr) {
     attach_next(d);
     // the kernel is instantiated for 1/2/4/8 columns: cover n with the largest pieces
     int done = 0;
@@ -155,7 +168,7 @@ static int mmvq_cols(b200q_mmvq_desc & d, int n, int64_t x_stride, cudaStream_t 
         if (c > max_cols) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)d.K);
         d.ncols = c; d.x = x0 + (int64_t)done * xs; d.x_stride = xs;
         for (int i = 0; i < d.n_seg; ++i) d.seg[i].dst = dst0[i] + (int64_t)done * d.seg[i].M;
-        int rc = check_launch(b200q_launch_mmvq(d, st), what);
+        int rc = check_launch(b200q_launch_mmvq(d, st, plan), what);
         if (rc) return rc;
         d.next = nullptr;
         done += c;
@@ -166,26 +179,23 @@ static int mmvq_cols(b200q_mmvq_desc & d, int n, int64_t x_stride, cudaStream_t 
 int b200q_mul_mat_vec(int type, const void * W, const float * x, float * dst, int64_t m, int64_t k, int n, int64_t x_stride,
                       const float * bias, void * stream) {
     if (!W || !x || !dst || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_vec: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_vec: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst, bias, m}; d.K = k; d.x = x; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_mul_mat_vec")) return rc;
+    d.n_seg = 1; d.seg[0] = {W, nullptr, dst, bias, m};
     return mmvq_cols(d, n, x_stride, (cudaStream_t)stream, "b200q_mul_mat_vec");
 }
 int b200q_mul_mat_vec_multi(int type, int n_tensors, const void * const * W, float * const * dst, const int64_t * m, int64_t k,
                             const float * x, int n, int64_t x_stride, void * stream) {
     if (n_tensors < 1 || n_tensors > B200Q_MAX_SEGS || !W || !dst || !m || !x || n < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_multi: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_vec_multi: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = n_tensors; d.K = k; d.x = x; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_mul_mat_vec_multi")) return rc;
+    d.n_seg = n_tensors;
     for (int i = 0; i < n_tensors; ++i) d.seg[i] = {W[i], nullptr, dst[i], nullptr, m[i]};
     return mmvq_cols(d, n, x_stride, (cudaStream_t)stream, "b200q_mul_mat_vec_multi");
 }
 int b200q_fused_up_gate_vec(int type, const void * W_up, const void * W_gate, const float * x, float * dst, int64_t m, int64_t k, int n,
                             int64_t x_stride, int unary, float limit, void * stream) {
     if (!W_up || !W_gate || !x || !dst || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_fused_up_gate_vec: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_fused_up_gate_vec: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = 1; d.seg[0] = {W_up, W_gate, dst, nullptr, m}; d.K = k; d.x = x; d.act = unary; d.limit = limit; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_fused_up_gate_vec")) return rc;
+    d.n_seg = 1; d.seg[0] = {W_up, W_gate, dst, nullptr, m}; d.act = unary; d.limit = limit;
     return mmvq_cols(d, n, x_stride, (cudaStream_t)stream, "b200q_fused_up_gate_vec");
 }
 
@@ -201,28 +211,21 @@ int b200q_fused_up_gate_vec_q8(int type, const void * W_up, const void * W_gate,
                                int unary, float limit, void * q8_out, int * q8_produced, void * stream) {
     if (q8_produced) *q8_produced = 0;
     if (!W_up || !W_gate || !x || !dst || m <= 0) return fail(B200Q_E_ARG, "b200q_fused_up_gate_vec_q8: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_fused_up_gate_vec_q8: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = 1; d.seg[0] = {W_up, W_gate, dst, nullptr, m}; d.K = k; d.x = x; d.x_stride = k; d.ncols = 1; d.act = unary; d.limit = limit;
-    d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
-    if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_fused_up_gate_vec_q8: activations must be 16-byte aligned");
-    attach_next(d);
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_fused_up_gate_vec_q8")) return rc;
+    d.n_seg = 1; d.seg[0] = {W_up, W_gate, dst, nullptr, m}; d.act = unary; d.limit = limit;
     if (q8_out && opt_q8()) d.q8_out = q8_out;     // a shape not eligible for the hand-off is planned as the plain launch
     b200q_mmvq_plan p;
-    const int rc = check_launch(b200q_launch_mmvq(d, (cudaStream_t)stream, &p), "b200q_fused_up_gate_vec_q8");
+    const int rc = mmvq_cols(d, 1, 0, (cudaStream_t)stream, "b200q_fused_up_gate_vec_q8", &p);
     if (rc == 0 && q8_produced) *q8_produced = p.q8 == 2;
     return rc;
 }
 int b200q_mul_mat_vec_q8(int type, const void * W, const float * x, const void * q8_in, float * dst, int64_t m, int64_t k,
                          const float * bias, void * stream) {
     if (!W || !x || !dst || m <= 0) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_q8: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_vec_q8: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst, bias, m}; d.K = k; d.x = x; d.x_stride = k; d.ncols = 1; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
-    if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_q8: activations must be 16-byte aligned");
-    attach_next(d);
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_mul_mat_vec_q8")) return rc;
+    d.n_seg = 1; d.seg[0] = {W, nullptr, dst, bias, m};
     if (q8_in && opt_q8()) d.q8_in = q8_in;
-    return check_launch(b200q_launch_mmvq(d, (cudaStream_t)stream), "b200q_mul_mat_vec_q8");
+    return mmvq_cols(d, 1, 0, (cudaStream_t)stream, "b200q_mul_mat_vec_q8");
 }
 
 int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const void * W_gate, float * const * dst, const int64_t * m,
@@ -239,9 +242,9 @@ int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const 
         return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: incomplete communicator");
     if (!reduce_in && !x) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: x is NULL");
     if (!reduce_out && !dst) return fail(B200Q_E_ARG, "b200q_mul_mat_vec_tp: dst is NULL");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_vec_tp: no CUDA device");
-    b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-    d.type = type; d.n_seg = n_tensors; d.K = k; d.x = x; d.x_stride = k; d.ncols = 1; d.act = unary; d.limit = limit; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = 1;
+    // launched directly, not through mmvq_cols: x may be NULL (reduce_in), and the launch does not consume a b200q_decode_prefetch_next hint
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, "b200q_mul_mat_vec_tp")) return rc;
+    d.n_seg = n_tensors; d.x_stride = k; d.ncols = 1; d.act = unary; d.limit = limit; d.ring = 1;
     for (int i = 0; i < n_tensors; ++i) d.seg[i] = {W[i], i == 0 ? W_gate : nullptr, dst ? dst[i] : nullptr, nullptr, m[i]};
     if (comm) {
         d.tp.ll_mc = (float2 *)comm->ll_mc; d.tp.ll_local = (const float2 *)comm->ll_local; d.tp.ll_red = (float2 *)comm->ll_reduced; d.tp.ll_stride = comm->ll_stride;
@@ -259,18 +262,18 @@ int b200q_mul_mat_vec_tp(int type, int n_tensors, const void * const * W, const 
 int b200q_reduce_sum_nvls(const float * in, float * out, int64_t n, void * mc_base, void * local_base, int64_t parity_stride,
                           void * mc_flag, const void * local_flag, uint32_t world_size, void * seq_counter, void * cta_counter, void * stream) {
     if (!in || !out || !mc_base || !local_base || !mc_flag || !local_flag || !seq_counter || !cta_counter || world_size < 2) return fail(B200Q_E_ARG, "b200q_reduce_sum_nvls: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_reduce_sum_nvls: no CUDA device");
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_reduce_sum_nvls")) return rc;
     return check_launch(b200q_launch_allreduce_nvls(in, out, n, mc_base, local_base, parity_stride, mc_flag, local_flag, world_size, seq_counter, cta_counter,
-                                                    di.sm_count, (cudaStream_t)stream), "b200q_reduce_sum_nvls");
+                                                    sms, (cudaStream_t)stream), "b200q_reduce_sum_nvls");
 }
 
 int b200q_reduce_sum_nvls_bf16(const float * in, float * out_f32, void * out_bf16, int64_t n, const b200q_nvls_stage * sg, void * stream) {
     if (!in || (!out_f32 && !out_bf16) || !sg || !sg->mc_stage || !sg->local_stage || !sg->mc_flag || !sg->local_flag || !sg->state || sg->world_size < 2 || sg->rank >= sg->world_size)
         return fail(B200Q_E_ARG, "b200q_reduce_sum_nvls_bf16: bad argument");
     if (n > sg->stage_elems || (n & 7)) return fail(B200Q_E_SHAPE, "b200q_reduce_sum_nvls_bf16: n must be a multiple of 8 and fit the staging buffer");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_reduce_sum_nvls_bf16: no CUDA device");
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_reduce_sum_nvls_bf16")) return rc;
     return check_launch(b200q_launch_allreduce_nvls_2shot(in, out_f32, out_bf16, n, sg->mc_stage, sg->local_stage, sg->mc_flag, sg->local_flag, sg->world_size, sg->rank,
-                                                          sg->state, di.sm_count, (cudaStream_t)stream), "b200q_reduce_sum_nvls_bf16");
+                                                          sg->state, sms, (cudaStream_t)stream), "b200q_reduce_sum_nvls_bf16");
 }
 
 size_t b200q_mul_mat_workspace(int type, int64_t m, int64_t k, int64_t n) { return n <= 8 ? 0 : b200q_gemm_workspace_bytes(type, m, k, n); }
@@ -283,8 +286,8 @@ int b200q_dequantize_bf16(int type, const void * W, void * out, int64_t m, int64
 int b200q_mul_mat_gemm(int type, const void * W, const float * x, float * dst, int64_t m, int64_t k, int64_t n,
                        void * workspace, size_t workspace_bytes, void * stream) {
     if (!W || !x || !dst || !workspace || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_gemm: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_gemm: no CUDA device");
-    return check_launch(b200q_launch_gemm(type, W, x, k, dst, m, k, n, workspace, workspace_bytes, di.sm_count, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm");
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_mul_mat_gemm")) return rc;
+    return check_launch(b200q_launch_gemm(type, W, x, k, dst, m, k, n, workspace, workspace_bytes, sms, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm");
 }
 int b200q_convert_f32_bf16(const float * x, int64_t x_stride, void * out_bf16, int64_t k, int64_t n, void * stream) {
     if (!x || !out_bf16 || n < 1) return fail(B200Q_E_ARG, "b200q_convert_f32_bf16: bad argument");
@@ -293,51 +296,50 @@ int b200q_convert_f32_bf16(const float * x, int64_t x_stride, void * out_bf16, i
 int b200q_mul_mat_gemm_bf16(int type, const void * W, const void * x_bf16, float * dst, int64_t m, int64_t k, int64_t n,
                             void * workspace, size_t workspace_bytes, void * stream) {
     if (!W || !x_bf16 || !dst || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_gemm_bf16: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_gemm_bf16: no CUDA device");
-    return check_launch(b200q_launch_gemm_bf16x(type, W, x_bf16, dst, m, k, n, workspace, workspace_bytes, di.sm_count, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm_bf16");
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_mul_mat_gemm_bf16")) return rc;
+    return check_launch(b200q_launch_gemm_bf16x(type, W, x_bf16, dst, m, k, n, workspace, workspace_bytes, sms, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm_bf16");
 }
 int b200q_mul_mat_gemm_multi_bf16(int type, int n_tensors, const void * const * W, float * const * dst, const int64_t * m, int64_t k,
                                   const void * x_bf16, int64_t n, void * workspace, size_t workspace_bytes, void * stream) {
     if (n_tensors < 1 || n_tensors > 3 || !W || !dst || !m || !x_bf16 || n < 1) return fail(B200Q_E_ARG, "b200q_mul_mat_gemm_multi_bf16: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_mul_mat_gemm_multi_bf16: no CUDA device");
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_mul_mat_gemm_multi_bf16")) return rc;
     b200q_gemm_multi d; memset(&d, 0, sizeof d);
     d.type = type; d.n_seg = n_tensors; d.K = k; d.N = n; d.xb = x_bf16;
     for (int i = 0; i < n_tensors; ++i) { if (!W[i] || !dst[i] || m[i] <= 0) return fail(B200Q_E_ARG, "b200q_mul_mat_gemm_multi_bf16: bad tensor %d", i); d.W[i] = W[i]; d.dst[i] = dst[i]; d.M[i] = m[i]; }
-    return check_launch(b200q_launch_gemm_multi_bf16x(d, workspace, workspace_bytes, di.sm_count, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm_multi_bf16");
+    return check_launch(b200q_launch_gemm_multi_bf16x(d, workspace, workspace_bytes, sms, opt_fused(), (cudaStream_t)stream), "b200q_mul_mat_gemm_multi_bf16");
 }
+// the largest tensor's rows: its bf16 weight scratch serves every tensor
+static int64_t max_rows(int n, const int64_t * m) { int64_t r = 0; for (int i = 0; m && i < n; ++i) r = m[i] > r ? m[i] : r; return r; }
 size_t b200q_mul_mat_multi_workspace(int type, int n_tensors, const int64_t * m, int64_t k, int64_t n) {
-    if (n <= 8 || !m) return 0;
-    int64_t mm = 0; for (int i = 0; i < n_tensors; ++i) mm = m[i] > mm ? m[i] : mm;
-    return b200q_gemm_workspace_bytes(type, mm, k, n);
+    return n <= 8 || !m ? 0 : b200q_gemm_workspace_bytes(type, max_rows(n_tensors, m), k, n);
 }
 int b200q_mul_mat_multi(int type, int n_tensors, const void * const * W, float * const * dst, const int64_t * m, int64_t k,
                         const float * x, int64_t n, void * workspace, size_t workspace_bytes, void * stream) {
     if (n <= 8) return b200q_mul_mat_vec_multi(type, n_tensors, W, dst, m, k, x, (int)n, k, stream);
     if (!x || !workspace) return fail(B200Q_E_ARG, "b200q_mul_mat_multi: bad argument");
     if (workspace_bytes < b200q_mul_mat_multi_workspace(type, n_tensors, m, k, n)) return fail(B200Q_E_NOMEM, "b200q_mul_mat_multi: workspace too small");
-    int rc = b200q_convert_f32_bf16(x, k, workspace, k, n, stream); if (rc) return rc;
-    const size_t off = (size_t)b200q_align_up(n * k * 2, 256);
-    return b200q_mul_mat_gemm_multi_bf16(type, n_tensors, W, dst, m, k, workspace, n, (char *)workspace + off, workspace_bytes - off, stream);
+    const b200q_dense_ws L = b200q_dense_layout(B200Q_DENSE_GEMM, max_rows(n_tensors, m), k, n);
+    char * ws = (char *)workspace;
+    if (const int rc = b200q_convert_f32_bf16(x, k, ws + L.x, k, n, stream)) return rc;
+    return b200q_mul_mat_gemm_multi_bf16(type, n_tensors, W, dst, m, k, ws + L.x, n, ws + L.wsc, workspace_bytes - L.wsc, stream);
 }
 
 size_t b200q_fused_up_gate_workspace(int type, int64_t m, int64_t k, int64_t n) {
-    if (n <= 8) return 0;
-    (void)type;     // bf16 activations + f32 up result + bf16 weight scratch (types without a fused kernel)
-    return (size_t)b200q_align_up(n * k * 2, 256) + (size_t)b200q_align_up(m * n * 4, 256) + (size_t)b200q_align_up(m * k * 2, 256);
+    (void)type;
+    return n <= 8 ? 0 : b200q_dense_layout(B200Q_DENSE_UP_GATE, m, k, n).total;
 }
-// x already bf16 [n][k]; workspace >= align(m*n*4) + align(m*k*2)
 int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_gate, const void * x_bf16, float * dst, void * dst_bf16,
                                   int64_t m, int64_t k, int64_t n, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
     if (!W_up || !W_gate || !x_bf16 || !dst || !workspace || m <= 0 || n < 1) return fail(B200Q_E_ARG, "b200q_fused_up_gate_gemm_bf16: bad argument");
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "b200q_fused_up_gate_gemm_bf16: no CUDA device");
-    const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
-    if (workspace_bytes < up_bytes) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate_gemm_bf16: workspace too small");
-    float * up_res = (float *)workspace; void * wsc = (char *)workspace + up_bytes; const size_t wsc_bytes = workspace_bytes - up_bytes;
-    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0; if (const int rc = device_sms(sms, "b200q_fused_up_gate_gemm_bf16")) return rc;
+    // the up result must fit; the launch checks the weight scratch, which only the types without a fused kernel use
+    const b200q_dense_ws L = b200q_dense_layout(B200Q_DENSE_UP_GATE_BF16, m, k, n);
+    if (workspace_bytes < L.wsc) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate_gemm_bf16: workspace too small");
+    float * up_res = (float *)((char *)workspace + L.up); cudaStream_t st = (cudaStream_t)stream;
     // up and gate as the two segments of ONE launch (up -> workspace, gate -> dst), then the unary-mul tail in place, which also writes dst_bf16
     b200q_gemm_multi d; memset(&d, 0, sizeof d);
     d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n; d.xb = x_bf16;
-    const int rc = check_launch(b200q_launch_gemm_multi_bf16x(d, wsc, wsc_bytes, di.sm_count, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(up,gate)");
+    const int rc = check_launch(b200q_launch_gemm_multi_bf16x(d, (char *)workspace + L.wsc, workspace_bytes - L.wsc, sms, opt_fused(), st), "b200q_fused_up_gate_gemm_bf16(up,gate)");
     if (rc) return rc;
     return check_launch(b200q_launch_mul_unary(dst, up_res, dst, dst_bf16, m * n, unary, limit, st), "b200q_fused_up_gate_gemm_bf16(unary)");
 }
@@ -347,19 +349,21 @@ int b200q_fused_up_gate(int type, const void * W_up, const void * W_gate, const 
     if (!x || !workspace) return fail(B200Q_E_ARG, "b200q_fused_up_gate: bad argument");
     if (workspace_bytes < b200q_fused_up_gate_workspace(type, m, k, n)) return fail(B200Q_E_NOMEM, "b200q_fused_up_gate: workspace too small");
     if ((m * n) % 4) return fail(B200Q_E_SHAPE, "b200q_fused_up_gate: m*n must be a multiple of 4");
+    char * ws = (char *)workspace;
     // ternary weights: both GEMMs on the int8 tensor pipe (one activation quantisation, one launch over the up and gate row tiles), then the unary-mul tail
-    const size_t up_bytes = (size_t)b200q_align_up(m * n * 4, 256);
-    if (opt_fused() && device_info().ok && b200q_gemm_bn_i8_ok(type, k, n, x, k, workspace_bytes - up_bytes)) {
-        float * up_res = (float *)workspace;
+    const b200q_dense_ws Li = b200q_dense_layout(B200Q_DENSE_UP_GATE_I8, m, k, n);
+    if (opt_fused() && device_info().ok && b200q_gemm_bn_i8_ok(type, k, n, x, k, workspace_bytes - Li.x)) {
+        float * up_res = (float *)(ws + Li.up);
         b200q_gemm_multi d; memset(&d, 0, sizeof d);
         d.type = type; d.n_seg = 2; d.W[0] = W_up; d.dst[0] = up_res; d.M[0] = m; d.W[1] = W_gate; d.dst[1] = dst; d.M[1] = m; d.K = k; d.N = n;
-        const int rc = check_launch(b200q_launch_gemm_bn_i8(d, x, k, (char *)workspace + up_bytes, workspace_bytes - up_bytes, (cudaStream_t)stream), "b200q_fused_up_gate(int8)");
+        const int rc = check_launch(b200q_launch_gemm_bn_i8(d, x, k, ws + Li.x, workspace_bytes - Li.x, (cudaStream_t)stream), "b200q_fused_up_gate(int8)");
         if (rc) return rc;
         return check_launch(b200q_launch_mul_unary(dst, up_res, dst, nullptr, m * n, unary, limit, (cudaStream_t)stream), "b200q_fused_up_gate(unary)");
     }
-    int rc = b200q_convert_f32_bf16(x, k, workspace, k, n, stream); if (rc) return rc;
-    const size_t off = (size_t)b200q_align_up(n * k * 2, 256);
-    return b200q_fused_up_gate_gemm_bf16(type, W_up, W_gate, workspace, dst, nullptr, m, k, n, unary, limit, (char *)workspace + off, workspace_bytes - off, stream);
+    // X, then the workspace of b200q_fused_up_gate_gemm_bf16 (B200Q_DENSE_UP_GATE_BF16)
+    const b200q_dense_ws L = b200q_dense_layout(B200Q_DENSE_UP_GATE, m, k, n);
+    if (const int rc = b200q_convert_f32_bf16(x, k, ws + L.x, k, n, stream)) return rc;
+    return b200q_fused_up_gate_gemm_bf16(type, W_up, W_gate, ws + L.x, dst, nullptr, m, k, n, unary, limit, ws + L.up, workspace_bytes - L.up, stream);
 }
 int b200q_mul_mat(int type, const void * W, const float * x, float * dst, int64_t m, int64_t k, int64_t n,
                   void * workspace, size_t workspace_bytes, void * stream) {
@@ -382,13 +386,20 @@ static void moe_desc(b200q_mmvq_id_desc & d, int type, const moe_operands & o, i
     d.M = m; d.K = k; d.n_expert = n_expert; d.n_used = n_used; d.nb1 = nb1; d.act = unary; d.limit = limit;
     d.x_tok_stride = (int64_t)nb1 * k; d.x_col_stride = k;      // MoE activations are contiguous; b200q_mul_mat_batched overrides both
 }
+// the argument checks of both bodies, in this order: operands (and the grouped path's workspace), device, the mat-vec's activation alignment
+// (the grouped GEMM's launch checks its own), token / slot counts
+static int moe_check(bool grouped, const moe_operands & o, const int32_t * ids, const float * x, const float * dst, const void * workspace,
+                     int64_t m, int64_t k, int n_expert, int n_used, int nb1, int n_tokens, int & sms, const char * what) {
+    if (!o.W || !ids || !x || !dst || (grouped && !workspace) || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
+    if (const int rc = device_sms(sms, what)) return rc;
+    if (!grouped && (((uintptr_t)x & 15) || (k & 3))) return fail(B200Q_E_ARG, "%s: activations must be 16-byte aligned", what);
+    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
+    return B200Q_OK;
+}
 static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst,
                    int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * stream, const char * what,
                    int64_t xs_tok = 0, int64_t xs_col = 0) {
-    if (!o.W || !ids || !x || !dst || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
-    if (((uintptr_t)x & 15) || (k & 3)) return fail(B200Q_E_ARG, "%s: activations must be 16-byte aligned", what);
-    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
+    int sms = 0; if (const int rc = moe_check(false, o, ids, x, dst, nullptr, m, k, n_expert, n_used, nb1, n_tokens, sms, what)) return rc;
     // the quantised activation columns of a launch live in shared memory: larger batches are walked in token chunks (same kernel, the expert ids
     // never leave the device).  Prefill batches are served by the grouped GEMM (b200q_mul_mat_id_gemm) once b200q_mul_mat_id selects it.
     int chunk = (int)(b200q_mmvq_max_cols(k) / nb1);
@@ -400,7 +411,7 @@ static int moe_vec(int type, const moe_operands & o, int n_expert, const int32_t
         b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
         if (xs_tok) { d.x_tok_stride = xs_tok; d.x_col_stride = xs_col; }
         d.ids = ids + (int64_t)t0 * n_used; d.x = x + (int64_t)t0 * d.x_tok_stride; d.dst = dst + (int64_t)t0 * n_used * m; d.n_tokens = nt;
-        d.sm_count = di.sm_count; d.pdl = opt_pdl();
+        d.sm_count = sms; d.pdl = opt_pdl();
         const int rc = check_launch(b200q_launch_mmvq_id(d, (cudaStream_t)stream), what);
         if (rc) return rc;
     }
@@ -421,26 +432,31 @@ int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate, int n_ex
  * Merged up/gate experts run the same launches on the same bytes as the split form, so they share its crossover. */
 static constexpr int64_t MOE_UP_GATE_MIN_ROWS_PER_EXPERT = 5;
 static constexpr int64_t MOE_MUL_MAT_ID_MIN_SLOTS = 32;
-static size_t moe_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate, int64_t rows_layout) {
-    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate)) return 0;
+// the crossover above: whether b200q_mul_mat_id takes the grouped GEMM for a shape the GEMM accepts
+static bool moe_grouped_pays(int n_used, int n_tokens, int n_expert, int up_gate) {
     const int64_t n_slots = (int64_t)n_tokens * n_used;
-    if (up_gate ? n_slots <= MOE_UP_GATE_MIN_ROWS_PER_EXPERT * n_expert : n_slots <= MOE_MUL_MAT_ID_MIN_SLOTS) return 0;
-    return b200q_moe_gemm_workspace_bytes(type, m, k, n_slots, n_expert, up_gate, rows_layout);
+    return n_slots > (up_gate ? MOE_UP_GATE_MIN_ROWS_PER_EXPERT * n_expert : MOE_MUL_MAT_ID_MIN_SLOTS);
+}
+// the grouped path's workspace, 0 for a shape it refuses
+static size_t moe_gemm_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate, int64_t rows_layout) {
+    if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate)) return 0;
+    return b200q_moe_gemm_workspace_bytes(type, m, k, (int64_t)n_tokens * n_used, n_expert, up_gate, rows_layout);
+}
+size_t b200q_mul_mat_id_gemm_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate) {
+    return moe_gemm_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate, m);
 }
 size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate) {
-    return moe_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate, m);
+    return moe_grouped_pays(n_used, n_tokens, n_expert, up_gate) ? b200q_mul_mat_id_gemm_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, up_gate) : 0;
 }
 static int moe_gemm(int type, const moe_operands & o, int n_expert, const int32_t * ids, const float * x, float * dst, int64_t m, int64_t k,
                     int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream, const char * what,
                     int64_t xs_tok = 0, int64_t xs_col = 0) {
-    if (!o.W || !ids || !x || !dst || !workspace || m <= 0 || n_expert < 1) return fail(B200Q_E_ARG, "%s: bad argument", what);
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
-    if (n_tokens < 1 || n_used < 1 || nb1 < 1 || n_used % nb1) return fail(B200Q_E_ARG, "%s: bad token / slot counts", what);
+    int sms = 0; if (const int rc = moe_check(true, o, ids, x, dst, workspace, m, k, n_expert, n_used, nb1, n_tokens, sms, what)) return rc;
     if (!b200q_moe_gemm_shape_ok(type, m, k, n_used, nb1, n_tokens, n_expert, o.W_gate != nullptr))
         return fail(B200Q_E_SHAPE, "%s: shape not supported by the grouped GEMM (K %% 256, n_expert <= 1024, type)", what);
     b200q_mmvq_id_desc d; moe_desc(d, type, o, n_expert, m, k, n_used, nb1, unary, limit);
     if (xs_tok) { d.x_tok_stride = xs_tok; d.x_col_stride = xs_col; }
-    d.ids = ids; d.x = x; d.dst = dst; d.n_tokens = n_tokens; d.sm_count = di.sm_count;
+    d.ids = ids; d.x = x; d.dst = dst; d.n_tokens = n_tokens; d.sm_count = sms;
     return check_launch(b200q_launch_moe_gemm(d, workspace, workspace_bytes, (cudaStream_t)stream), what);
 }
 int b200q_mul_mat_id_gemm(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
@@ -457,8 +473,8 @@ int b200q_mul_mat_id(int type, const void * W, const void * W_gate, int n_expert
 
 /* MOE_FUSED_UP_GATE over merged experts: W_gate_up holds n_expert matrices [2 m x k], gate rows [0, m) then up rows [m, 2 m) */
 size_t b200q_moe_up_gate_merged_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert) {
-    if (m < 1 || m > INT32_MAX / 4) return 0;
-    return moe_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, 1, 2 * m);
+    if (m < 1 || m > INT32_MAX / 4 || !moe_grouped_pays(n_used, n_tokens, n_expert, 1)) return 0;
+    return moe_gemm_workspace(type, m, k, n_used, nb1, n_tokens, n_expert, 1, 2 * m);
 }
 int b200q_moe_up_gate_merged(int type, const void * W_gate_up, int n_expert, const int32_t * ids, const float * x, float * dst,
                              int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream) {
@@ -547,21 +563,20 @@ int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float *
     batched_plan p;
     if (const int rc = plan_batched(type, m, k, n, n_batch, per_entry, x_col_stride, x_batch_stride, p, what)) return rc;
     if (workspace_bytes < p.ws_bytes || (p.ws_bytes && !workspace)) return fail(B200Q_E_NOMEM, "%s: workspace too small", what);
-    dev_info & di = device_info(); if (!di.ok) return fail(B200Q_E_CUDA, "%s: no CUDA device", what);
+    int sms = 0; if (const int rc = device_sms(sms, what)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (p.path == BATCHED_ONE) {
         if (p.n_cols <= 8) {
-            b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-            d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst, nullptr, m}; d.K = k; d.x = x; d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+            b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x, what)) return rc;
+            d.n_seg = 1; d.seg[0] = {W, nullptr, dst, nullptr, m};
             return mmvq_cols(d, (int)p.n_cols, p.x_stride, st, what);
         }
-        return check_launch(b200q_launch_gemm(type, W, x, p.x_stride, dst, m, k, p.n_cols, workspace, workspace_bytes, di.sm_count, opt_fused(), st), what);
+        return check_launch(b200q_launch_gemm(type, W, x, p.x_stride, dst, m, k, p.n_cols, workspace, workspace_bytes, sms, opt_fused(), st), what);
     }
     if (p.path == BATCHED_ENTRY_VEC) {  // the broadcast matrix, one dense mat-vec per entry over its strided columns
         for (int b = 0; b < n_batch; ++b) {
-            b200q_mmvq_desc d; memset(&d, 0, sizeof d);
-            d.type = type; d.n_seg = 1; d.seg[0] = {W, nullptr, dst + (int64_t)b * n * m, nullptr, m}; d.K = k; d.x = x + b * x_batch_stride;
-            d.sm_count = di.sm_count; d.pdl = opt_pdl(); d.ring = opt_ring();
+            b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, x + b * x_batch_stride, what)) return rc;
+            d.n_seg = 1; d.seg[0] = {W, nullptr, dst + (int64_t)b * n * m, nullptr, m};
             if (const int rc = mmvq_cols(d, (int)n, x_col_stride, st, what)) return rc;
         }
         return B200Q_OK;
@@ -570,7 +585,7 @@ int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float *
         const int64_t wstride = per_entry ? b200q_plane_bytes(type, m, k) : 0;
         for (int b = 0; b < n_batch; ++b) {
             const int rc = check_launch(b200q_launch_gemm(type, (const char *)W + b * wstride, x + b * x_batch_stride, x_col_stride, dst + (int64_t)b * n * m, m, k, n,
-                                                          workspace, workspace_bytes, di.sm_count, opt_fused(), st), what);
+                                                          workspace, workspace_bytes, sms, opt_fused(), st), what);
             if (rc) return rc;
         }
         return B200Q_OK;

@@ -820,9 +820,19 @@ int b200q_launch_mul_unary(const float * gate, const float * up, float * dst, vo
     return (int)cudaGetLastError();
 }
 
+b200q_dense_ws b200q_dense_layout(int kind, int64_t M, int64_t K, int64_t N) {
+    b200q_dense_ws L{}; size_t off = 0;
+    auto take = [&](int64_t bytes) { const size_t o = off; off += (size_t)b200q_align_up(bytes, 256); return o; };
+    if (kind == B200Q_DENSE_GEMM || kind == B200Q_DENSE_UP_GATE) L.x = take(N * K * 2);
+    if (kind >= B200Q_DENSE_UP_GATE) L.up = take(M * N * 4);
+    if (kind == B200Q_DENSE_UP_GATE_I8) L.x = take((int64_t)b200q_gemm_i8_workspace_bytes(K, N));
+    else L.wsc = take(M * K * 2);
+    L.total = off;
+    return L;
+}
 size_t b200q_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t N) {
     (void)type;
-    return (size_t)b200q_align_up(N * K * 2, 256) + (size_t)b200q_align_up(M * K * 2, 256);
+    return b200q_dense_layout(B200Q_DENSE_GEMM, M, K, N).total;
 }
 
 // f32 [N][K] -> bf16 [N][K] (shared by the mat-muls that consume the same activation)
@@ -861,7 +871,7 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
     // Every segment's type and scratch size is checked before the first memset or launch: an error return leaves every dst untouched.
     for (int i = 0; i < d.n_seg; ++i) {
         b200q_layout L; if (b200q_make_layout(type, d.M[i], K, &L)) return -1;
-        if (ws_bytes < (size_t)b200q_align_up(d.M[i] * K * 2, 256)) return -5;
+        if (ws_bytes < b200q_dense_layout(B200Q_DENSE_GEMM_BF16, d.M[i], K, N).total) return -5;
     }
     for (int i = 0; i < d.n_seg; ++i) {
         const int64_t M = d.M[i];
@@ -931,17 +941,17 @@ int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * d
     return b200q_launch_gemm_multi_bf16x(d, wscratch, ws_bytes, sm_count, fused, st);
 }
 
-// A = planes of `type` [M][K]; X = f32 [N][K]; dst f32 [N][M].  Workspace: bf16 X followed by bf16 W (unfused path only).
+// A = planes of `type` [M][K]; X = f32 [N][K]; dst f32 [N][M].  Workspace: B200Q_DENSE_GEMM.
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
                       void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st) {
-    if (ws_bytes < b200q_gemm_workspace_bytes(type, M, K, N)) return -5;
-    if (fused && b200q_gemm_bn_i8_ok(type, K, N, x, x_stride, ws_bytes)) {     // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
+    const b200q_dense_ws L = b200q_dense_layout(B200Q_DENSE_GEMM, M, K, N);
+    if (ws_bytes < L.total) return -5;
+    if (fused && b200q_gemm_bn_i8_ok(type, K, N, x, x_stride, ws_bytes - L.x)) {     // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
         b200q_gemm_multi d; memset(&d, 0, sizeof d);
         d.type = type; d.n_seg = 1; d.W[0] = W; d.dst[0] = dst; d.M[0] = M; d.K = K; d.N = N;
-        return b200q_launch_gemm_bn_i8(d, x, x_stride, ws, ws_bytes, st);
+        return b200q_launch_gemm_bn_i8(d, x, x_stride, (char *)ws + L.x, ws_bytes - L.x, st);
     }
-    void * xb = ws;
-    void * wb = (char *)ws + b200q_align_up(N * K * 2, 256);
+    void * xb = (char *)ws + L.x;
     int rc = b200q_launch_f32_to_bf16(x, x_stride, xb, K, N, st); if (rc) return rc;
-    return b200q_launch_gemm_bf16x(type, W, xb, dst, M, K, N, wb, ws_bytes - (size_t)b200q_align_up(N * K * 2, 256), sm_count, fused, st);
+    return b200q_launch_gemm_bf16x(type, W, xb, dst, M, K, N, (char *)ws + L.wsc, ws_bytes - L.wsc, sm_count, fused, st);
 }

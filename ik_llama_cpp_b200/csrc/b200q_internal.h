@@ -91,7 +91,19 @@ struct b200q_gemm_multi {
     int type; int n_seg; const void * W[3]; float * dst[3]; int64_t M[3];
     int64_t K, N; const void * xb;
 };
-size_t b200q_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t N);
+// Workspace of the dense prefill entry points: byte offsets of its regions, in the order listed, each 256-byte aligned.  An absent region has
+// offset 0.  X: bf16 [N][K] activations, or the int8 image of the IQ2_BN path (b200q_gemm_i8_workspace_bytes), which may use the bytes after it;
+// up: f32 [N][M] up result; wsc: bf16 [M][K] weight scratch of the types without a fused kernel.
+enum {
+    B200Q_DENSE_GEMM,            // X | wsc      b200q_launch_gemm, b200q_mul_mat_multi (M: the largest tensor)
+    B200Q_DENSE_GEMM_BF16,       // wsc          X given in bf16: b200q_launch_gemm_multi_bf16x, per tensor
+    B200Q_DENSE_UP_GATE,         // X | up | wsc b200q_fused_up_gate
+    B200Q_DENSE_UP_GATE_BF16,    // up | wsc     b200q_fused_up_gate_gemm_bf16
+    B200Q_DENSE_UP_GATE_I8,      // up | X       b200q_fused_up_gate on the int8 path
+};
+struct b200q_dense_ws { size_t x, up, wsc, total; };
+b200q_dense_ws b200q_dense_layout(int kind, int64_t M, int64_t K, int64_t N);
+size_t b200q_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t N);     // B200Q_DENSE_GEMM's total
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
                       void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * dst, int64_t M, int64_t K, int64_t N,

@@ -94,7 +94,8 @@ B200Q_API int b200q_decode_prefetch_next(int type, int n_tensors, const void * c
 B200Q_API size_t b200q_mul_mat_workspace(int type, int64_t m, int64_t k, int64_t n);
 B200Q_API int b200q_mul_mat_gemm(int type, const void * W, const float * x, float * dst, int64_t m, int64_t k, int64_t n,
                        void * workspace, size_t workspace_bytes, void * stream);
-/* activations shared by several mat-muls (Q,K,V / up,gate): convert once, then call the _bf16 variant per weight tensor */
+/* activations shared by several mat-muls (Q,K,V / up,gate): convert once, then call the _bf16 variant per weight tensor.  A workspace of
+ * b200q_mul_mat_workspace (b200q_mul_mat_multi_workspace for _multi_bf16) bytes is always enough for it. */
 B200Q_API int b200q_convert_f32_bf16(const float * x, int64_t x_stride, void * out_bf16, int64_t k, int64_t n, void * stream);
 B200Q_API int b200q_mul_mat_gemm_bf16(int type, const void * W, const void * x_bf16, float * dst, int64_t m, int64_t k, int64_t n,
                             void * workspace /* bf16 [m][k] scratch, only for types without a fused kernel */, size_t workspace_bytes, void * stream);
@@ -106,7 +107,8 @@ B200Q_API int b200q_mul_mat_gemm_multi_bf16(int type, int n_tensors, const void 
 /* GGML_OP_FUSED_UP_GATE for n > 8 (ggml_cuda_up_gate_unary, ggml-cuda.cu:3588-3618: two MMQ + ggml_fused_mul_unary): up and gate
  * are the two segments of one GEMM launch, followed by one elementwise unary-mul pass; dst_bf16 (optional, may be NULL) receives a
  * bf16 copy = the operand of ffn_down.
- * workspace >= align256(m*n*4) (the up result) + align256(m*k*2) (the bf16 weight scratch, only for types without a fused kernel) */
+ * workspace >= align256(m*n*4) (the up result) + align256(m*k*2) (the bf16 weight scratch, only for types without a fused kernel);
+ * b200q_fused_up_gate_workspace bytes are always enough */
 B200Q_API int b200q_fused_up_gate_gemm_bf16(int type, const void * W_up, const void * W_gate, const void * x_bf16, float * dst, void * dst_bf16,
                                   int64_t m, int64_t k, int64_t n, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);
 
@@ -186,10 +188,12 @@ B200Q_API int b200q_mul_mat_id_vec(int type, const void * W, const void * W_gate
  * Same arguments and result as b200q_mul_mat_id_vec, plus a device workspace.  Routing (counts, sort by expert, tile table) runs on the device: no
  * host round trip, no allocation, no synchronisation, so the call can be captured in a CUDA graph.  Ids outside [0, n_expert) are skipped and their
  * dst rows are ZERO (the reference's semantics, as in b200q_mul_mat_id_vec).  bf16 operands, f32 accumulation (as the dense GEMM).
- * b200q_mul_mat_id_workspace: bytes the grouped path needs, or 0 exactly when b200q_mul_mat_id takes the mat-vec path: an ineligible shape, or a
- * batch below the measured crossover (n_slots = n_tokens * n_used; up/gate: n_slots <= 5 * n_expert, else n_slots <= 32).  Needs no device.
+ * b200q_mul_mat_id_gemm_workspace: bytes b200q_mul_mat_id_gemm needs at any batch size, 0 only for a shape the grouped path refuses.  Needs no device.
+ * b200q_mul_mat_id_workspace: the same bytes where b200q_mul_mat_id takes the grouped path, 0 exactly when it takes the mat-vec path: an ineligible
+ * shape, or a batch below the measured crossover (n_slots = n_tokens * n_used; up/gate: n_slots <= 5 * n_expert, else n_slots <= 32).  Needs no device.
  * b200q_mul_mat_id_gemm: always the grouped path (K % 256 == 0, n_expert <= 1024).  b200q_mul_mat_id: the dispatcher (workspace may be NULL when the
  * query returned 0). */
+B200Q_API size_t b200q_mul_mat_id_gemm_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate);
 B200Q_API size_t b200q_mul_mat_id_workspace(int type, int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int n_expert, int up_gate);
 B200Q_API int b200q_mul_mat_id_gemm(int type, const void * W, const void * W_gate, int n_expert, const int32_t * ids, const float * x, float * dst,
                           int64_t m, int64_t k, int n_used, int nb1, int n_tokens, int unary, float limit, void * workspace, size_t workspace_bytes, void * stream);

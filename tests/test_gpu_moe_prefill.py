@@ -126,6 +126,25 @@ def test_grouped_equals_dense_gemm_per_expert(be, oracle, name):
     assert checked >= 6
 
 
+def test_grouped_gemm_below_the_crossover(be, oracle):
+    """mul_mat_id_gemm runs the grouped GEMM at any batch, also where the dispatcher takes the mat-vec and b200q_mul_mat_id_workspace is 0:
+    3 experts, 1 used, 4 tokens.  Its workspace comes from b200q_mul_mat_id_gemm_workspace.  The result matches mul_mat_id (the mat-vec kernel)
+    within the two paths' noise, as test_gpu_parity.py::test_gemm_llama_shape_properties, and the exact product within the grouped GEMM's bar."""
+    name = "IQ4_NL"
+    n_expert, n_used, m, k, n_tokens = 3, 1, 256, 2048, 4
+    wires, W = experts(be, oracle, name, n_expert, m, k, 1900)
+    rng = np.random.default_rng(19)
+    x = rng.standard_normal((n_tokens, 1, k)).astype(np.float32)
+    ids = np.array([[0], [2], [1], [2]], np.int32)
+    assert be.mul_mat_id_workspace(W, n_tokens, n_used, 1, False) == 0
+    be._workspaces.clear()          # sized by this call's own query, not by an earlier test's larger workspace
+    xg, idg = torch.from_numpy(x).cuda(), torch.from_numpy(ids).cuda()
+    y = be.mul_mat_id_gemm(W, xg, idg).cpu().numpy()
+    yv = be.mul_mat_id(W, xg, idg).cpu().numpy()
+    assert nmse(y, yv) <= 1e-4
+    assert nmse(y, exact(oracle, name, wires, None, x, ids, m)) <= 2e-5
+
+
 @pytest.mark.parametrize("name", ["IQ4_NL", "Q6_K"])
 @pytest.mark.parametrize("n_expert,n_tokens", [(256, 600), (8, 1100)])
 def test_skewed_routing_and_skipped_ids(be, oracle, name, n_expert, n_tokens):

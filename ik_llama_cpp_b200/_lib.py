@@ -97,6 +97,11 @@ def lib() -> ctypes.CDLL:
         L.b200q_mul_mat_batched_workspace.restype = c_size_t
         L.b200q_mul_mat_batched_workspace.argtypes = [i32, i64, i64, i64, i32, i32, i64, i64]
         L.b200q_mul_mat_batched.argtypes = [i32, vp, i32, vp, i64, i64, vp, i64, i64, i64, i32, vp, c_size_t, vp]
+    if hasattr(L, "b200q_mul_mat_rows"):
+        L.b200q_mul_mat_rows_ok.argtypes = [i32, i64, i64, i64, i64, i64, i32, i64]
+        L.b200q_mul_mat_rows_workspace.restype = c_size_t
+        L.b200q_mul_mat_rows_workspace.argtypes = [i32, i64, i64, i64, i64, i64, i32, i64]
+        L.b200q_mul_mat_rows.argtypes = [i32, vp, i64, i64, i32, vp, i64, vp, i64, i64, i64, vp, c_size_t, vp]
     if hasattr(L, "b200q_decode_prefetch_next"):
         L.b200q_decode_prefetch_next.argtypes = [i32, i32, vp, vp, vp, i64]
     _lib = L

@@ -402,6 +402,35 @@ def mul_mat_batched(w: "QuantTensor | ExpertTensor", x_view: torch.Tensor, per_e
     return dst
 
 
+_X_TYPES = {torch.float32: 0, torch.float16: 1}      # ggml_type ids of the activations of mul_mat_rows
+
+
+def mul_mat_rows_workspace(w: QuantTensor, row0: int, m: int, n: int, x_dtype: torch.dtype, x_col_stride: int) -> int:
+    """Bytes of device workspace mul_mat_rows needs (b200q_mul_mat_rows_workspace; no device needed; 0 for a rejected argument)."""
+    return int(_lib.lib().b200q_mul_mat_rows_workspace(w.ggml_type, w.m, row0, m, w.k, n, _X_TYPES[x_dtype], x_col_stride))
+
+
+def mul_mat_rows(w: QuantTensor, x: torch.Tensor, row0: int, m: int, out: torch.Tensor | None = None) -> torch.Tensor:
+    """GGML_OP_MUL_MAT over the rows [row0, row0 + m) of the whole weight w (b200q_mul_mat_rows): dst f32 [N, m] = x [N, K] times those rows.
+    x: a 2-D f32 or f16 CUDA tensor with stride(1) == 1 (a view with columns further apart, such as DeepSeek's f16 K cache without its rope part,
+    is read in place)."""
+    if x.dim() != 2 or x.dtype not in _X_TYPES or x.shape[1] != w.k or x.stride(1) != 1:
+        raise ValueError(f"mul_mat_rows: x must be f32 or f16 [N, K={w.k}] with contiguous rows, got {x.dtype} {tuple(x.shape)} strides {x.stride()}")
+    _require_cuda()
+    if not x.is_cuda:
+        raise ValueError("mul_mat_rows: x must be a CUDA tensor")
+    n, cs = x.shape[0], x.stride(0)
+    dst = out if out is not None else torch.empty((n, m), dtype=torch.float32, device=x.device)
+    assert dst.dtype == torch.float32 and dst.is_contiguous() and dst.shape == (n, m)
+    need = mul_mat_rows_workspace(w, row0, m, n, x.dtype, cs)
+    L = _lib.lib()
+    with torch.cuda.device(x.device):
+        ws = _workspace(need, x.device) if need else None
+        check(L.b200q_mul_mat_rows(w.ggml_type, w.ptr, w.m, row0, _X_TYPES[x.dtype], x.data_ptr(), cs, dst.data_ptr(), m, w.k, n,
+                                   ws.data_ptr() if ws is not None else None, ws.numel() if ws is not None else 0, _stream()), "b200q_mul_mat_rows")
+    return dst
+
+
 def moe_combine(rows: torch.Tensor, weights: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
     """GGML_OP_MUL_MULTI_ADD (b200q_moe_combine): rows f32 [n_tokens, n_used, M], weights f32 [n_tokens, n_used] -> dst f32 [n_tokens, M],
     dst[t] = sum_u weights[t, u] * rows[t, u], summed in slot order in f32 as the reference CPU op."""

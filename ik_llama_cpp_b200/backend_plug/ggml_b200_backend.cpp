@@ -2,7 +2,7 @@
 //
 // Implements the reference's backend vtable (struct ggml_backend_i, ggml/src/ggml-backend-impl.h:81-130) and buffer vtables
 // (:18-51) on top of libb200q.so, and exports the C symbols of ggml/include/ggml-cuda.h:24-46 under their original names.
-// graph_compute owns the hot path: GGML_OP_MUL_MAT on block-quantized src0 (2-D and batched), GGML_OP_FUSED_UP_GATE, the MoE ops (MUL_MAT_ID,
+// graph_compute owns the hot path: GGML_OP_MUL_MAT on block-quantized src0 (2-D, batched, and over whole-row views of a weight with f32 or f16 src1), GGML_OP_FUSED_UP_GATE, the MoE ops (MUL_MAT_ID,
 // MOE_FUSED_UP_GATE and the MUL_MULTI_ADD that combines the routed experts, so a MoE FFN never leaves the device), the look-ahead
 // fusions of ggml_cuda_mul_mat_q (Q,K,V sharing src1; a trailing bias ADD, ggml-cuda.cu:2573-2601) and the q8_1 hand-off from
 // FUSED_UP_GATE to the following MUL_MAT (ffn_down).  Every other op is reported as unsupported (supports_op == false): this library is the
@@ -275,6 +275,25 @@ static bool b200_can_mul_mat(const ggml_tensor * w, const ggml_tensor * x, const
     if (!(w->ne[2] == 1 || (w->ne[2] == x->ne[2] && x->ne[3] == 1))) return false;
     return x->ne[2] * x->ne[3] > 1 ? b200_batched_x(x, nullptr, nullptr) : ggml_is_contiguous(x);
 }
+// MUL_MAT through b200q_mul_mat_rows, for nodes b200_can_mul_mat declines (those keep their path): src0 a whole plug weight or a view of whole rows
+// of a 2-D one (DeepSeek's pp_opt wkv_b_iter, build_deepseek2.cpp:971-972), src1 2-D f32 or f16 with contiguous rows a multiple of 16 bytes apart (the
+// f16 K cache view kv_cache_nope, :924-925).  The library's check decides which row origins keep the planes aligned.  Returns the whole weight, the
+// slice's first row and src1's column stride in elements.
+static bool b200_can_mul_mat_rows(const ggml_tensor * w, const ggml_tensor * x, const ggml_tensor * dst, const ggml_tensor ** parent, int64_t * row0, int64_t * cs) {
+    if (!w || !x || dst->type != GGML_TYPE_F32 || !ggml_is_contiguous(dst) || w->ne[0] != x->ne[0] || w->ne[2] != 1 || w->ne[3] != 1) return false;
+    const ggml_tensor * p = w; int64_t r0 = 0;
+    if (!b200_weight_ok(w)) {
+        p = w->view_src;
+        if (!p || !b200_weight_ok(p) || p->ne[2] != 1 || w->type != p->type || w->ne[0] != p->ne[0] || w->nb[1] != p->nb[1] || w->view_offs % p->nb[1]) return false;
+        r0 = (int64_t)(w->view_offs / p->nb[1]);
+    }
+    if ((x->type != GGML_TYPE_F32 && x->type != GGML_TYPE_F16) || x->ne[2] != 1 || x->ne[3] != 1) return false;
+    const size_t es = ggml_type_size(x->type);
+    if (x->nb[0] != es || (x->view_offs & 15) || (x->nb[1] & 15) || x->nb[1] < x->ne[0] * es) return false;
+    if (b200q_mul_mat_rows_ok(w->type, p->ne[1], r0, w->ne[1], w->ne[0], x->ne[1], x->type, (int64_t)(x->nb[1] / es)) != 0) return false;
+    if (parent) { *parent = p; *row0 = r0; *cs = (int64_t)(x->nb[1] / es); }
+    return true;
+}
 // MoE expert ids: int32 [n_used, n_tokens], consecutive within a token.  The tokens' rows may lie further apart: ggml_top_k returns a view of the
 // argsort result (nb1 = n_expert * 4), and the scheduler's copy keeps that layout; graph_compute gathers such rows into its workspace.
 static bool b200_ids_ok(const ggml_tensor * ids) {
@@ -284,7 +303,7 @@ static bool b200_ids_strided(const ggml_tensor * ids) { return ids->ne[1] > 1 &&
 GGML_CALL static bool b200_backend_supports_op(ggml_backend_t, const ggml_tensor * op) {
     switch (op->op) {
         case GGML_OP_NONE: case GGML_OP_RESHAPE: case GGML_OP_VIEW: case GGML_OP_PERMUTE: case GGML_OP_TRANSPOSE: return true;
-        case GGML_OP_MUL_MAT: return b200_can_mul_mat(op->src[0], op->src[1], op);
+        case GGML_OP_MUL_MAT: return b200_can_mul_mat(op->src[0], op->src[1], op) || b200_can_mul_mat_rows(op->src[0], op->src[1], op, nullptr, nullptr, nullptr);
         case GGML_OP_ADD:       // the bias of a mat-mul result ([M] broadcast over the columns) or a same-shape f32 add, on our buffers
             return op->type == GGML_TYPE_F32 && op->src[0] && op->src[1] && op->src[0]->type == GGML_TYPE_F32 && op->src[1]->type == GGML_TYPE_F32 &&
                    ggml_is_contiguous(op) && ggml_is_contiguous(op->src[0]) && ggml_is_contiguous(op->src[1]) && ggml_are_same_shape(op, op->src[0]) &&
@@ -328,7 +347,14 @@ GGML_CALL static enum ggml_status b200_backend_graph_compute(ggml_backend_t b, g
             case GGML_OP_NONE: case GGML_OP_RESHAPE: case GGML_OP_VIEW: case GGML_OP_PERMUTE: case GGML_OP_TRANSPOSE: break;
             case GGML_OP_MUL_MAT: {
                 const ggml_tensor * w = node->src[0]; const ggml_tensor * x = node->src[1];
-                GGML_ASSERT(b200_can_mul_mat(w, x, node));
+                if (!b200_can_mul_mat(w, x, node)) {    // a row slice of a weight and / or an f16 or strided src1: on its own, never in a look-ahead fusion
+                    const ggml_tensor * p = nullptr; int64_t row0 = 0, cs = 0;
+                    GGML_ASSERT(b200_can_mul_mat_rows(w, x, node, &p, &row0, &cs));
+                    const size_t need = b200q_mul_mat_rows_workspace(w->type, p->ne[1], row0, w->ne[1], w->ne[0], x->ne[1], x->type, cs);
+                    void * ws = need ? c->workspace(need) : nullptr;
+                    B200Q_CHECK(b200q_mul_mat_rows(w->type, p->data, p->ne[1], row0, x->type, x->data, cs, (float *)node->data, w->ne[1], w->ne[0], x->ne[1], ws, need, c->stream));
+                    break;
+                }
                 const int64_t m = w->ne[1], k = w->ne[0], n = x->ne[1];
                 const int64_t nbatch = x->ne[2] * x->ne[3];
                 if (nbatch > 1) {       // batched / broadcast MUL_MAT over a strided src1 (src0 broadcast over the batch or one matrix per entry)

@@ -79,14 +79,15 @@ def build_backend_plug(force: bool = False, verbose: bool = False) -> str | None
 
 
 BACKEND_OPS_TESTS = ["test_mul_mat_backend", "test_moe_prefill_backend", "test_plug_graphs", "test_moe_merged_backend", "test_moe_combine_backend",
-                     "test_plug_mla"]
+                     "test_plug_mla", "test_plug_mla_pp"]
 
 
 def build_backend_ops_test(force: bool = False) -> str | None:
     """tests/backend_ops/test_mul_mat_backend (returned) and test_moe_prefill_backend: test-backend-ops semantics through the real ggml-backend API;
     test_plug_graphs: model-shaped graphs through ggml_backend_sched, dumped node by node; test_moe_merged_backend: merged up/gate MoE experts
     against the reference CPU backend, as a node and inside the MoE FFN graph; test_moe_combine_backend: MUL_MULTI_ADD, as a node and ending the
-    fused_mmad MoE FFN graph."""
+    fused_mmad MoE FFN graph; test_plug_mla: DeepSeek's batched MLA products; test_plug_mla_pp: its prompt-processing wkv_b product over row slices
+    of the weight and the f16 K cache."""
     root = os.path.dirname(HERE)
     exes = [os.path.join(root, "tests", "backend_ops", name) for name in BACKEND_OPS_TESTS]
     if not os.path.isdir(REFERENCE_ROOT):

@@ -598,6 +598,55 @@ int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float *
                     x_batch_stride, x_col_stride);
 }
 
+/* MUL_MAT over a row slice of a weight uploaded whole, over f32 or f16 activations a column stride apart (include/b200q.h).  The row origin is
+ * resolved on the host into the plane pointers / tensor maps of the launches b200q_mul_mat makes; f16 activations are converted once: widened to
+ * f32 for the mat-vec (its prologue quantises from f32) and the IQ2_BN int8 GEMM, to bf16 for every other GEMM. */
+static constexpr int X_F32 = 0, X_F16 = 1;      // ggml_type ids of the activations
+static int rows_check(int type, int64_t rows_layout, int64_t row0, int64_t m, int64_t k, int64_t n, int x_type, int64_t cs, const char * what) {
+    if (x_type != X_F32 && x_type != X_F16) return fail(B200Q_E_TYPE, "%s: activations must be f32 or f16", what);
+    b200q_layout P;
+    if (const int rc = b200q_make_layout(type, rows_layout < 1 ? 1 : rows_layout, k, &P))
+        return rc == -1 ? fail(B200Q_E_TYPE, "%s: unsupported ggml type", what) : fail(B200Q_E_SHAPE, "%s: k = %lld is not a multiple of the type's block", what, (long long)k);
+    if (rows_layout < 1 || m < 1 || n < 1 || row0 < 0 || row0 > rows_layout - m) return fail(B200Q_E_ARG, "%s: rows [row0, row0 + m) must lie in the tensor", what);
+    const int64_t es = x_type == X_F16 ? 2 : 4;
+    if (cs < 0 || (cs * es) % 16 || (n > 1 && cs < k)) return fail(B200Q_E_ARG, "%s: x_col_stride must be a multiple of 16 bytes, at least k when n > 1", what);
+    if (P.wire > 1 && (row0 % P.wire || m % P.wire)) return fail(B200Q_E_SHAPE, "%s: row0 and m must be multiples of %d for this type (its rows are interleaved)", what, P.wire);
+    for (int p = 0; p < B200Q_MAX_PLANES; ++p)      // every plane pointer of the slice keeps the 256-byte alignment of a whole tensor's
+        if (b200q_row_offset(P, p, row0) % 256) return fail(B200Q_E_SHAPE, "%s: row %lld does not start a 256-byte aligned row in plane %d", what, (long long)row0, p);
+    if (n > INT32_MAX) return fail(B200Q_E_SHAPE, "%s: too many columns", what);
+    if (n <= 8 && b200q_mmvq_max_cols(k) < 1) return fail(B200Q_E_SHAPE, "%s: K=%lld too large for the mat-vec kernel", what, (long long)k);
+    return B200Q_OK;
+}
+int b200q_mul_mat_rows_ok(int type, int64_t rows_layout, int64_t row0, int64_t m, int64_t k, int64_t n, int x_type, int64_t x_col_stride) {
+    return rows_check(type, rows_layout, row0, m, k, n, x_type, x_col_stride, "b200q_mul_mat_rows_ok");
+}
+size_t b200q_mul_mat_rows_workspace(int type, int64_t rows_layout, int64_t row0, int64_t m, int64_t k, int64_t n, int x_type, int64_t x_col_stride) {
+    if (rows_check(type, rows_layout, row0, m, k, n, x_type, x_col_stride, "b200q_mul_mat_rows_workspace")) return 0;
+    if (n <= 8) return x_type == X_F16 ? (size_t)b200q_align_up(n * k * 4, 256) : 0;
+    const bool widen = x_type == X_F16 && b200q_gemm_bn_i8_ok(type, k, n, nullptr, k, SIZE_MAX);
+    return b200q_dense_layout(widen ? B200Q_DENSE_GEMM_WIDEN : B200Q_DENSE_GEMM, m, k, n).total;
+}
+int b200q_mul_mat_rows(int type, const void * W, int64_t rows_layout, int64_t row0, int x_type, const void * x, int64_t x_col_stride,
+                       float * dst, int64_t m, int64_t k, int64_t n, void * workspace, size_t workspace_bytes, void * stream) {
+    static const char * what = "b200q_mul_mat_rows";
+    if (!W || !x || !dst || ((uintptr_t)x & 15) || ((uintptr_t)workspace & 255)) return fail(B200Q_E_ARG, "%s: bad argument (x 16-byte, workspace 256-byte aligned)", what);
+    if (const int rc = rows_check(type, rows_layout, row0, m, k, n, x_type, x_col_stride, what)) return rc;
+    const size_t need = b200q_mul_mat_rows_workspace(type, rows_layout, row0, m, k, n, x_type, x_col_stride);
+    if (workspace_bytes < need || (need && !workspace)) return fail(B200Q_E_NOMEM, "%s: workspace too small", what);
+    int sms = 0; if (const int rc = device_sms(sms, what)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n > 8) return check_launch(b200q_launch_gemm_rows(type, W, rows_layout, row0, x, x_type == X_F16, x_col_stride, dst, m, k, n, workspace, workspace_bytes,
+                                                          sms, opt_fused(), st), what);
+    const float * xf = (const float *)x; int64_t xs = x_col_stride;
+    if (x_type == X_F16) {
+        if (const int rc = check_launch(b200q_launch_f16_convert(x, x_col_stride, workspace, 0, k, n, st), what)) return rc;
+        xf = (const float *)workspace; xs = k;
+    }
+    b200q_mmvq_desc d; if (const int rc = mmvq_desc(d, type, k, xf, what)) return rc;
+    d.n_seg = 1; d.seg[0] = {W, nullptr, dst, nullptr, m, rows_layout, row0};
+    return mmvq_cols(d, (int)n, xs, st, what);
+}
+
 int b200q_mul_mat_host(int type, const void * W, const float * x_host, float * dst_host, int64_t m, int64_t k, int64_t n, void * stream) {
     cudaStream_t st = (cudaStream_t)stream; cudaError_t e; int rc;
     const size_t xb = (size_t)n * k * sizeof(float), yb = (size_t)n * m * sizeof(float), wsb = b200q_mul_mat_workspace(type, m, k, n);

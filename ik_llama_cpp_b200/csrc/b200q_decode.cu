@@ -104,7 +104,7 @@ int b200q_launch_dequant_bf16(const void * W, const b200q_layout & L, void * out
 }
 int b200q_launch_dequant_bf16_experts(const void * W, const b200q_layout & L, void * out, int e0, int n_e, const int * bounds, cudaStream_t st) {
     if (n_e < 1 || n_e > 65535) return -2;
-    if (L.wire) return b200q_launch_wire_dequant_bf16_experts(L.type, W, L.M, L.K, L.total_bytes, out, e0, n_e, bounds, st);
+    if (L.wire) return b200q_launch_wire_dequant_bf16_experts(L.type, (const uint8_t *)W + L.plane_off[0], L.M, L.K, L.total_bytes, out, e0, n_e, bounds, st);
     const int64_t total = L.M * (L.K / 32);
     const int bs = 256; int64_t nb = (total + bs - 1) / bs; const int64_t cap = 132 * 64 / n_e > 1 ? 132 * 64 / n_e : 1; if (nb > cap) nb = cap; if (nb < 1) nb = 1;
     const dim3 grid((unsigned)nb, (unsigned)n_e);
@@ -356,7 +356,8 @@ int b200q_launch_mmvq(const b200q_mmvq_desc & d, cudaStream_t st, b200q_mmvq_pla
     if (g_trace && g_trace_slot < 4096) { if (g_trace_cta && g_trace_slot < 512) a.trace_cta = g_trace_cta + (size_t)g_trace_slot * 2048; a.trace = g_trace + 8 * (g_trace_slot++); }
     int64_t r0 = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        b200q_layout L; b200q_make_layout(d.type, d.seg[i].M, d.K, &L);
+        const b200q_mmvq_seg_desc & sg = d.seg[i];
+        b200q_layout L; if (b200q_slice_layout(d.type, sg.rows_layout ? sg.rows_layout : sg.M, sg.w_row0, sg.M, d.K, &L)) return -2;
         a.seg[i].P = b200q_planes_from((const uint8_t *)d.seg[i].W, L);
         if (d.seg[i].W2) a.seg[i].P2 = b200q_planes_from((const uint8_t *)d.seg[i].W2, L);
         a.seg[i].dst = d.seg[i].dst; a.seg[i].bias = d.seg[i].bias; a.seg[i].M = d.seg[i].M; a.seg[i].row0 = r0; r0 += d.seg[i].M;

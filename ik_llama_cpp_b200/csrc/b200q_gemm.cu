@@ -15,11 +15,13 @@
 #include "b200q_decode_plan.h"
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <climits>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <mutex>
 
 namespace {
@@ -647,6 +649,33 @@ __global__ void k_f32_to_bf16_k4(const float * __restrict__ x, int64_t xs, __nv_
     }
 }
 
+// f16 [N][K] (row stride xs halves) -> OUT [N][K] (bf16, or f32 to widen), E = 8 halves per item (one 16-byte load, one 16-byte bf16 store or two
+// f32 ones) or, for K % 8 != 0, 4.  Both outputs are exact images of float(x): widening f16 is exact, and bf16(f16) rounds the same real value as
+// bf16(f32(f16)), so the products that follow give the bits of the same call over f32 activations holding float(x).
+template <typename OUT, int E>
+__global__ void __launch_bounds__(256) k_f16_convert(const __half * __restrict__ x, int64_t xs, OUT * __restrict__ out, int64_t K, int64_t N) {
+    using V = typename std::conditional<E == 8, uint4, uint2>::type;
+    const int64_t ke = K / E, total = N * ke;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t n = i / ke, c = i % ke;
+        const V v = __ldg(reinterpret_cast<const V *>(x + n * xs + E * c));
+        const uint32_t * w = reinterpret_cast<const uint32_t *>(&v);
+        float f[E];
+#pragma unroll
+        for (int j = 0; j < E / 2; ++j) { const float2 t = __half22float2(*reinterpret_cast<const __half2 *>(w + j)); f[2 * j] = t.x; f[2 * j + 1] = t.y; }
+        OUT * o = out + n * K + E * c;
+        if constexpr (std::is_same<OUT, float>::value) {
+#pragma unroll
+            for (int q = 0; q < E / 4; ++q) reinterpret_cast<float4 *>(o)[q] = make_float4(f[4 * q], f[4 * q + 1], f[4 * q + 2], f[4 * q + 3]);
+        } else {
+            V r; uint32_t * rw = reinterpret_cast<uint32_t *>(&r);
+#pragma unroll
+            for (int j = 0; j < E / 2; ++j) { const __nv_bfloat162 b = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]); rw[j] = *reinterpret_cast<const uint32_t *>(&b); }
+            *reinterpret_cast<V *>(o) = r;
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // host side: tensor maps
 // ---------------------------------------------------------------------------------------------------------------
@@ -707,19 +736,19 @@ constexpr bool gemmq_supported(int type) {
 }
 
 // k_gemm_q over the segments of d.  GROUPED: d.W[i] holds n_mat expert matrices (one 3-D map per plane covers them all) and blockIdx.y walks
-// the tile table of rt.  rows: when not null, segment i is the row range [rows->row0[i], rows->row0[i] + d.M[i]) of matrices of rows->rows_layout
-// rows (merged up/gate experts): its maps start at that row and end after d.M[i] rows, so a partial last tile is zero-filled, not the next range
+// the tile table of rt.  Segment i is the row range [d.row0[i], d.row0[i] + d.M[i]) of matrices of d.rows_layout rows (merged up/gate experts, a
+// row slice of a dense weight): its maps start at that row and end after d.M[i] rows, so a partial last tile is zero-filled, not the next range
 template <int TYPE, int NB, bool GROUPED>
-int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, const b200q_moe_gemm * rows, cudaStream_t st) {
+int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, cudaStream_t st) {
     using cfg = typename gemmq_policy<TYPE, NB, GROUPED>::cfg;
     gemm_decode_args<cfg::N_PLANES> a; memset(&a, 0, sizeof a);
     const int box[3] = {128, cfg::P1, cfg::P2};                   // bytes per row of each plane per 256 weights
     int tiles = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        b200q_layout L; if (b200q_make_layout(TYPE, rows ? rows->rows_layout : d.M[i], d.K, &L)) return -1;
+        b200q_layout L; if (b200q_make_layout(TYPE, d.rows_layout ? d.rows_layout : d.M[i], d.K, &L)) return -1;
         for (int p = 0; p < cfg::N_PLANES; ++p) {
             const int64_t row_bytes = (d.K / 256) * box[p];
-            const char * base = (const char *)d.W[i] + L.plane_off[p] + (rows ? b200q_row_offset(L, p, rows->row0[i]) : 0);
+            const char * base = (const char *)d.W[i] + L.plane_off[p] + b200q_row_offset(L, p, d.row0[i]);
             if (make_tmap(&a.tmP[p][i], TM_U8, GROUPED ? 3 : 2, base, {row_bytes, d.M[i], n_mat},
                                     {row_bytes, L.total_bytes}, {box[p], BM, 1}, p == 0)) return p == 0 ? -10 : -13;
         }
@@ -734,10 +763,9 @@ int launch_gemm_q(const b200q_gemm_multi & d, int k_split, int64_t n_mat, const 
     return (int)cudaGetLastError();
 }
 template <bool GROUPED>
-int launch_gemm_q(int type, bool bn256, const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, const b200q_moe_gemm * rows,
-                  cudaStream_t st) {
+int launch_gemm_q(int type, bool bn256, const b200q_gemm_multi & d, int k_split, int64_t n_mat, const b200q_moe_route & rt, cudaStream_t st) {
     switch (type) {
-#define X(T) case T: return bn256 ? launch_gemm_q<T, 1, GROUPED>(d, k_split, n_mat, rt, rows, st) : launch_gemm_q<T, 0, GROUPED>(d, k_split, n_mat, rt, rows, st);
+#define X(T) case T: return bn256 ? launch_gemm_q<T, 1, GROUPED>(d, k_split, n_mat, rt, st) : launch_gemm_q<T, 0, GROUPED>(d, k_split, n_mat, rt, st);
         GEMMQ_TYPES(X)
 #undef X
         default: return -1;
@@ -751,7 +779,7 @@ int launch_gemm_bn_i8(const b200q_gemm_multi & d, const int8_t * xq, const float
     gemm_decode_args<1> a; memset(&a, 0, sizeof a);
     int tiles = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        b200q_layout L; if (b200q_make_layout(B200Q_TYPE_IQ2_BN, d.M[i], d.K, &L)) return -1;
+        b200q_layout L; if (b200q_slice_layout(B200Q_TYPE_IQ2_BN, d.rows_layout ? d.rows_layout : d.M[i], d.row0[i], d.M[i], d.K, &L)) return -1;
         if (make_tmap(&a.tmP[0][i], TM_U8, 2, (const char *)d.W[i] + L.plane_off[0], {d.K / 4, d.M[i]}, {d.K / 4}, {128, BM}, true)) return -10;
         a.seg[i].dst = d.dst[i]; a.seg[i].rs = reinterpret_cast<const float *>((const char *)d.W[i] + L.plane_off[1]); a.seg[i].M = (int)d.M[i]; a.seg[i].tile0 = tiles;
         tiles += (int)((d.M[i] + BM - 1) / BM);
@@ -823,7 +851,8 @@ int b200q_launch_mul_unary(const float * gate, const float * up, float * dst, vo
 b200q_dense_ws b200q_dense_layout(int kind, int64_t M, int64_t K, int64_t N) {
     b200q_dense_ws L{}; size_t off = 0;
     auto take = [&](int64_t bytes) { const size_t o = off; off += (size_t)b200q_align_up(bytes, 256); return o; };
-    if (kind == B200Q_DENSE_GEMM || kind == B200Q_DENSE_UP_GATE) L.x = take(N * K * 2);
+    if (kind == B200Q_DENSE_GEMM_WIDEN) L.xf = take(N * K * 4);
+    if (kind == B200Q_DENSE_GEMM || kind == B200Q_DENSE_GEMM_WIDEN || kind == B200Q_DENSE_UP_GATE) L.x = take(N * K * 2);
     if (kind >= B200Q_DENSE_UP_GATE) L.up = take(M * N * 4);
     if (kind == B200Q_DENSE_UP_GATE_I8) L.x = take((int64_t)b200q_gemm_i8_workspace_bytes(K, N));
     else L.wsc = take(M * K * 2);
@@ -849,6 +878,22 @@ int b200q_launch_f32_to_bf16(const float * x, int64_t x_stride, void * out, int6
     return (int)cudaGetLastError();
 }
 
+int b200q_launch_f16_convert(const void * x, int64_t x_stride, void * out, int to_bf16, int64_t K, int64_t N, cudaStream_t st) {
+    const int64_t xs = x_stride ? x_stride : K;
+    if (K % 4 || xs % 4 || ((uintptr_t)x & 7) || ((uintptr_t)out & 7)) return -2;
+    const bool e8 = K % 8 == 0 && xs % 8 == 0 && !((uintptr_t)x & 15) && !((uintptr_t)out & 15);
+    const int64_t total = N * (K / (e8 ? 8 : 4)); int64_t nb = (total + 255) / 256; if (nb > 132 * 32) nb = 132 * 32; if (nb < 1) nb = 1;
+    const __half * h = (const __half *)x;
+    if (to_bf16) {
+        if (e8) k_f16_convert<__nv_bfloat16, 8><<<(unsigned)nb, 256, 0, st>>>(h, xs, (__nv_bfloat16 *)out, K, N);
+        else k_f16_convert<__nv_bfloat16, 4><<<(unsigned)nb, 256, 0, st>>>(h, xs, (__nv_bfloat16 *)out, K, N);
+    } else {
+        if (e8) k_f16_convert<float, 8><<<(unsigned)nb, 256, 0, st>>>(h, xs, (float *)out, K, N);
+        else k_f16_convert<float, 4><<<(unsigned)nb, 256, 0, st>>>(h, xs, (float *)out, K, N);
+    }
+    return (int)cudaGetLastError();
+}
+
 // n_seg weight tensors of one type and K sharing X = bf16 [N][K] (already converted); dst[i] f32 [N][M_i].
 // wscratch: bf16 W scratch (max M_i x K) for the unfused path.
 int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st) {
@@ -865,17 +910,19 @@ int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, s
         const int64_t tiles = mt * ((N + bn - 1) / bn);
         const int k_split = gemmq_choose_split(tiles, K / 256, sm_count);
         if (k_split > 1) for (int i = 0; i < d.n_seg; ++i) { cudaError_t e = cudaMemsetAsync(d.dst[i], 0, (size_t)d.M[i] * N * sizeof(float), st); if (e != cudaSuccess) return -3; }
-        return launch_gemm_q<false>(type, bn256, d, k_split, 1, b200q_moe_route{}, nullptr, st);
+        return launch_gemm_q<false>(type, bn256, d, k_split, 1, b200q_moe_route{}, st);
     }
     // unfused: bf16 weight scratch + plain bf16 GEMM per tensor; tile / split selection: fill ~1 wave of the SMs.
     // Every segment's type and scratch size is checked before the first memset or launch: an error return leaves every dst untouched.
+    // (a row slice dequantises only its own rows: its layout's plane offsets start at row0)
+    b200q_layout Ls[GEMMQ_MAX_SEGS];
     for (int i = 0; i < d.n_seg; ++i) {
-        b200q_layout L; if (b200q_make_layout(type, d.M[i], K, &L)) return -1;
+        if (b200q_slice_layout(type, d.rows_layout ? d.rows_layout : d.M[i], d.row0[i], d.M[i], K, &Ls[i])) return -1;
         if (ws_bytes < b200q_dense_layout(B200Q_DENSE_GEMM_BF16, d.M[i], K, N).total) return -5;
     }
     for (int i = 0; i < d.n_seg; ++i) {
         const int64_t M = d.M[i];
-        b200q_layout L; b200q_make_layout(type, M, K, &L);
+        const b200q_layout & L = Ls[i];
         const int64_t mt = (M + BM - 1) / BM;
         const bool bn256 = N >= 256 && mt * ((N + 255) / 256) >= sm_count / 2;
         const int64_t tiles = bn256 ? mt * ((N + 255) / 256) : mt * ((N + 127) / 128);
@@ -912,9 +959,9 @@ int b200q_launch_gemm_grouped(const b200q_moe_gemm & g, void * wscratch, size_t 
     const bool bn256 = g.bn == 256;
     if (gemmq_supported(g.type)) {
         b200q_gemm_multi d; memset(&d, 0, sizeof d);
-        d.type = g.type; d.n_seg = g.n_seg; d.K = g.K; d.N = g.n_rows; d.xb = g.xb;
-        for (int i = 0; i < g.n_seg; ++i) { d.W[i] = g.W[i]; d.dst[i] = g.dst[i]; d.M[i] = g.M; }
-        return launch_gemm_q<true>(g.type, bn256, d, 1, g.n_expert, g.rt, &g, st);
+        d.type = g.type; d.n_seg = g.n_seg; d.K = g.K; d.N = g.n_rows; d.xb = g.xb; d.rows_layout = g.rows_layout;
+        for (int i = 0; i < g.n_seg; ++i) { d.W[i] = g.W[i]; d.dst[i] = g.dst[i]; d.M[i] = g.M; d.row0[i] = g.row0[i]; }
+        return launch_gemm_q<true>(g.type, bn256, d, 1, g.n_expert, g.rt, st);
     }
     b200q_layout L; if (b200q_make_layout(g.type, g.rows_layout, g.K, &L)) return -1;
     const int64_t ebytes = g.rows_layout * g.K * 2;
@@ -944,14 +991,27 @@ int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * d
 // A = planes of `type` [M][K]; X = f32 [N][K]; dst f32 [N][M].  Workspace: B200Q_DENSE_GEMM.
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
                       void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st) {
-    const b200q_dense_ws L = b200q_dense_layout(B200Q_DENSE_GEMM, M, K, N);
+    return b200q_launch_gemm_rows(type, W, M, 0, x, 0, x_stride, dst, M, K, N, ws, ws_bytes, sm_count, fused, st);
+}
+// A = rows [row0, row0 + M) of the planes of `type` [rows_layout][K]: the activations become bf16 once (f16 ones by k_f16_convert, which replaces
+// k_f32_to_bf16), or, for IQ2_BN on the int8 pipe, are quantised from f32 (f16 ones widened first)
+int b200q_launch_gemm_rows(int type, const void * W, int64_t rows_layout, int64_t row0, const void * x, int x_f16, int64_t x_stride, float * dst,
+                           int64_t M, int64_t K, int64_t N, void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st) {
+    const bool widen = x_f16 && fused && b200q_gemm_bn_i8_ok(type, K, N, nullptr, K, SIZE_MAX);
+    const b200q_dense_ws L = b200q_dense_layout(widen ? B200Q_DENSE_GEMM_WIDEN : B200Q_DENSE_GEMM, M, K, N);
     if (ws_bytes < L.total) return -5;
-    if (fused && b200q_gemm_bn_i8_ok(type, K, N, x, x_stride, ws_bytes - L.x)) {     // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
-        b200q_gemm_multi d; memset(&d, 0, sizeof d);
-        d.type = type; d.n_seg = 1; d.W[0] = W; d.dst[0] = dst; d.M[0] = M; d.K = K; d.N = N;
-        return b200q_launch_gemm_bn_i8(d, x, x_stride, (char *)ws + L.x, ws_bytes - L.x, st);
+    char * w = (char *)ws;
+    b200q_gemm_multi d; memset(&d, 0, sizeof d);
+    d.type = type; d.n_seg = 1; d.W[0] = W; d.dst[0] = dst; d.M[0] = M; d.K = K; d.N = N; d.rows_layout = rows_layout; d.row0[0] = row0;
+    const float * xf = (const float *)x; int64_t xs = x_stride;
+    if (widen) {
+        if (const int rc = b200q_launch_f16_convert(x, x_stride, w + L.xf, 0, K, N, st)) return rc;
+        xf = (const float *)(w + L.xf); xs = K;
     }
-    void * xb = (char *)ws + L.x;
-    int rc = b200q_launch_f32_to_bf16(x, x_stride, xb, K, N, st); if (rc) return rc;
-    return b200q_launch_gemm_bf16x(type, W, xb, dst, M, K, N, (char *)ws + L.wsc, ws_bytes - L.wsc, sm_count, fused, st);
+    if (fused && (!x_f16 || widen) && b200q_gemm_bn_i8_ok(type, K, N, xf, xs, ws_bytes - L.x))     // ternary weights: int8 tensor pipe (u8 x s8 wgmma), exact integer accumulation
+        return b200q_launch_gemm_bn_i8(d, xf, xs, w + L.x, ws_bytes - L.x, st);
+    d.xb = w + L.x;
+    const int rc = x_f16 ? b200q_launch_f16_convert(x, x_stride, w + L.x, 1, K, N, st) : b200q_launch_f32_to_bf16(xf, x_stride, w + L.x, K, N, st);
+    if (rc) return rc;
+    return b200q_launch_gemm_multi_bf16x(d, w + L.wsc, ws_bytes - L.wsc, sm_count, fused, st);
 }

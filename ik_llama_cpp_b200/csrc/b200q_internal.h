@@ -57,7 +57,8 @@ struct b200q_tp_comm {
     uint32_t * seq;              // rank-local: [0] reduces issued by this rank, [1] CTA arrival counter
     int in; int out;
 };
-struct b200q_mmvq_seg_desc { const void * W; const void * W2; float * dst; const float * bias; int64_t M; };
+// w_row0 / rows_layout: the segment reads rows [w_row0, w_row0 + M) of W (and W2), tensors of rows_layout rows (0: M, a whole tensor)
+struct b200q_mmvq_seg_desc { const void * W; const void * W2; float * dst; const float * bias; int64_t M; int64_t rows_layout, w_row0; };
 struct b200q_mmvq_desc {
     int type; int n_seg; b200q_mmvq_seg_desc seg[B200Q_MAX_SEGS];
     int64_t K; const float * x; int64_t x_stride; int ncols; int act; float limit; int sm_count; int pdl; int ring;
@@ -86,26 +87,33 @@ int b200q_launch_wire_mmvq_id(const b200q_mmvq_id_desc & d, cudaStream_t st);
 // wire-layout types (b200q_wire.cu)
 int b200q_launch_wire_dequant_bf16(int type, const void * W, int64_t M, int64_t K, void * out, cudaStream_t st);
 
-// prefill: up to 3 weight tensors of one type / K that share the bf16 activation operand xb [N][K]
+// prefill: up to 3 weight tensors of one type / K that share the bf16 activation operand xb [N][K].  Segment i reads the rows
+// [row0[i], row0[i] + M[i]) of W[i], a tensor of rows_layout rows (0: M[i], a whole tensor)
 struct b200q_gemm_multi {
     int type; int n_seg; const void * W[3]; float * dst[3]; int64_t M[3];
     int64_t K, N; const void * xb;
+    int64_t rows_layout, row0[3];
 };
 // Workspace of the dense prefill entry points: byte offsets of its regions, in the order listed, each 256-byte aligned.  An absent region has
 // offset 0.  X: bf16 [N][K] activations, or the int8 image of the IQ2_BN path (b200q_gemm_i8_workspace_bytes), which may use the bytes after it;
 // up: f32 [N][M] up result; wsc: bf16 [M][K] weight scratch of the types without a fused kernel.
 enum {
     B200Q_DENSE_GEMM,            // X | wsc      b200q_launch_gemm, b200q_mul_mat_multi (M: the largest tensor)
+    B200Q_DENSE_GEMM_WIDEN,      // xf | X | wsc b200q_launch_gemm_rows with f16 activations on the int8 path (xf: them widened to f32 [N][K])
     B200Q_DENSE_GEMM_BF16,       // wsc          X given in bf16: b200q_launch_gemm_multi_bf16x, per tensor
     B200Q_DENSE_UP_GATE,         // X | up | wsc b200q_fused_up_gate
     B200Q_DENSE_UP_GATE_BF16,    // up | wsc     b200q_fused_up_gate_gemm_bf16
     B200Q_DENSE_UP_GATE_I8,      // up | X       b200q_fused_up_gate on the int8 path
 };
-struct b200q_dense_ws { size_t x, up, wsc, total; };
+struct b200q_dense_ws { size_t xf, x, up, wsc, total; };
 b200q_dense_ws b200q_dense_layout(int kind, int64_t M, int64_t K, int64_t N);
 size_t b200q_gemm_workspace_bytes(int type, int64_t M, int64_t K, int64_t N);     // B200Q_DENSE_GEMM's total
 int b200q_launch_gemm(int type, const void * W, const float * x, int64_t x_stride, float * dst, int64_t M, int64_t K, int64_t N,
                       void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
+// the same over rows [row0, row0 + M) of a tensor of rows_layout rows, x f32 or (x_f16) f16 [N][K] with a row stride of x_stride elements
+// (0: K).  Workspace: B200Q_DENSE_GEMM, or B200Q_DENSE_GEMM_WIDEN for f16 activations of a shape b200q_gemm_bn_i8_ok accepts
+int b200q_launch_gemm_rows(int type, const void * W, int64_t rows_layout, int64_t row0, const void * x, int x_f16, int64_t x_stride, float * dst,
+                           int64_t M, int64_t K, int64_t N, void * ws, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_gemm_bf16x(int type, const void * W, const void * xb, float * dst, int64_t M, int64_t K, int64_t N,
                             void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
 int b200q_launch_gemm_multi_bf16x(const b200q_gemm_multi & d, void * wscratch, size_t ws_bytes, int sm_count, int fused, cudaStream_t st);
@@ -116,6 +124,8 @@ bool b200q_gemm_bn_i8_ok(int type, int64_t K, int64_t N, const float * x, int64_
 int b200q_launch_gemm_bn_i8(const b200q_gemm_multi & d, const float * x, int64_t x_stride, void * ws, size_t ws_bytes, cudaStream_t st);
 int b200q_launch_add_rows(const float * a, const float * b, float * dst, int64_t m, int64_t n, int64_t nb, cudaStream_t st);
 int b200q_launch_f32_to_bf16(const float * x, int64_t x_stride, void * out, int64_t K, int64_t N, cudaStream_t st);
+// f16 [N][K] (row stride x_stride halves, 0: K) -> bf16 (to_bf16) or f32 [N][K]; both exact images of float(x)
+int b200q_launch_f16_convert(const void * x, int64_t x_stride, void * out, int to_bf16, int64_t K, int64_t N, cudaStream_t st);
 int b200q_gemm_fused_type(int type);
 
 // MoE prefill (b200q_moe.cu): routing tables of the expert-sorted slots, built on the device by k_moe_route and read by the grouped GEMMs.
@@ -151,6 +161,17 @@ int b200q_launch_moe_combine(const float * rows, const float * w, float * dst, i
 static inline int64_t b200q_row_offset(const b200q_layout & L, int p, int64_t row0) {
     if (L.wire) return p == 0 ? row0 * ((int64_t)L.row_meta + L.nb * L.wire_block) : 0;
     return row0 * (L.plane_per_row[p] ? 1 : L.nb) * L.plane_bytes[p];
+}
+// rows [row0, row0 + M) of a tensor of rows_layout rows as a layout of M rows over the tensor's base: plane p of the slice starts at plane_off[p]
+// (a wire-layout type's verbatim rows at plane_off[0]).  rows_layout = M, row0 = 0 gives b200q_make_layout's layout.  total_bytes stays the slice's
+// own (an expert stride, unused for one matrix).
+static inline int b200q_slice_layout(int type, int64_t rows_layout, int64_t row0, int64_t M, int64_t K, b200q_layout * S) {
+    b200q_layout P;
+    if (const int rc = b200q_make_layout(type, rows_layout, K, &P)) return rc;
+    if (const int rc = b200q_make_layout(type, M, K, S)) return rc;
+    if (row0 < 0 || row0 + M > rows_layout || (P.wire > 1 && row0 % P.wire)) return -2;
+    for (int p = 0; p < B200Q_MAX_PLANES; ++p) S->plane_off[p] = P.plane_off[p] + b200q_row_offset(P, p, row0);
+    return 0;
 }
 static inline b200q_planes b200q_planes_at(const uint8_t * base, const b200q_layout & L, int64_t row0) {
     b200q_planes P = b200q_planes_from(base, L);

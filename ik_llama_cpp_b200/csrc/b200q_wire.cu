@@ -211,9 +211,11 @@ int b200q_launch_wire_mmvq(const b200q_mmvq_desc & d, const b200q_mmvq_plan & p,
     wire_mmvq_args a; memset(&a, 0, sizeof a);
     int64_t r0 = 0;
     for (int i = 0; i < d.n_seg; ++i) {
-        a.W[i] = (const uint8_t *)d.seg[i].W; a.dst[i] = d.seg[i].dst; a.bias[i] = d.seg[i].bias; a.M[i] = d.seg[i].M; a.row0[i] = r0; r0 += d.seg[i].M;
+        const b200q_mmvq_seg_desc & sg = d.seg[i];
+        b200q_layout L; if (b200q_slice_layout(d.type, sg.rows_layout ? sg.rows_layout : sg.M, sg.w_row0, sg.M, d.K, &L)) return -2;
+        a.W[i] = (const uint8_t *)d.seg[i].W + L.plane_off[0]; if (i == 0 && sg.W2) a.W2 = (const uint8_t *)sg.W2 + L.plane_off[0];
+        a.dst[i] = d.seg[i].dst; a.bias[i] = d.seg[i].bias; a.M[i] = d.seg[i].M; a.row0[i] = r0; r0 += d.seg[i].M;
     }
-    a.W2 = (const uint8_t *)d.seg[0].W2;
     a.n_seg = d.n_seg; a.M_total = r0; a.K = d.K; a.x = d.x; a.x_stride = d.x_stride ? d.x_stride : d.K; a.act = d.act; a.limit = d.limit;
     const void * k = nullptr;
     switch (d.type) {

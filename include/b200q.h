@@ -238,6 +238,28 @@ B200Q_API size_t b200q_mul_mat_batched_workspace(int type, int64_t m, int64_t k,
                                                  int64_t x_col_stride, int64_t x_batch_stride);
 B200Q_API int b200q_mul_mat_batched(int type, const void * W, int per_entry, const float * x, int64_t x_col_stride, int64_t x_batch_stride,
                                     float * dst, int64_t m, int64_t k, int64_t n, int n_batch, void * workspace, size_t workspace_bytes, void * stream);
+/* ---- MUL_MAT over a row slice of a weight, over f32 or f16 activations a column stride apart ----
+ * (the "pp_opt" prompt processing of DeepSeek's MLA: kv_f32 = wkv_b_iter x kv_cache_nope, src/graphs/build_deepseek2.cpp:922-1022, where wkv_b_iter is a
+ * view of whole rows of wkv_b and kv_cache_nope a view of the f16 K cache, 576 halves per column starting 64 halves in)
+ *     dst[j][i] = W_row(row0 + i) . x[j * x_col_stride + 0 .. k)      i < m, j < n;  dst f32 contiguous [n][m]
+ * W is the base of the WHOLE tensor [rows_layout x k], uploaded with b200q_set_tensor (never a wire-byte offset into it); x_type is the ggml_type of x,
+ * GGML_TYPE_F32 (0) or GGML_TYPE_F16 (1); x_col_stride is in elements.
+ * Conditions:
+ *   - 0 <= row0, row0 + m <= rows_layout, n >= 1; x_col_stride a non-negative multiple of 16 bytes, at least k when n > 1 (otherwise B200Q_E_ARG);
+ *   - every plane pointer of the slice keeps the 256-byte alignment of a whole tensor's: row0 * (bytes per row of plane p) % 256 == 0 for every plane p
+ *     (a wire-layout type: row0 * wire row bytes % 256 == 0), and for the types whose rows are interleaved in groups of 4 (_R4) row0 % 4 == m % 4 == 0;
+ *     k a multiple of the type's block (otherwise B200Q_E_SHAPE);  an unsupported weight type or x_type: B200Q_E_TYPE;
+ *   - x 16-byte aligned, workspace 256-byte aligned (B200Q_E_ARG).
+ * Result: the launches of b200q_mul_mat on the rows [row0, row0 + m) uploaded as a tensor of their own, with the same bits (except launches that split
+ * K, whose f32 atomics may differ in the last bits from run to run); an f16 x gives the bits of an f32 x holding float(x).  The one extra launch for an
+ * f16 x converts it once: f16 -> f32 before a mat-vec (n <= 8) or the IQ2_BN int8 GEMM, f16 -> bf16 in place of f32 -> bf16 before every other GEMM.
+ * b200q_mul_mat_rows_ok: 0 or the B200Q_E_* the call would return for these arguments (before the pointer checks); needs no device.
+ * b200q_mul_mat_rows_workspace: the bytes the call needs (0 for a rejected argument, and for f32 x with n <= 8); needs no device.
+ * No host round trip, allocation or synchronisation: the call can be captured in a CUDA graph. */
+B200Q_API int    b200q_mul_mat_rows_ok(int type, int64_t rows_layout, int64_t row0, int64_t m, int64_t k, int64_t n, int x_type, int64_t x_col_stride);
+B200Q_API size_t b200q_mul_mat_rows_workspace(int type, int64_t rows_layout, int64_t row0, int64_t m, int64_t k, int64_t n, int x_type, int64_t x_col_stride);
+B200Q_API int    b200q_mul_mat_rows(int type, const void * W, int64_t rows_layout, int64_t row0, int x_type, const void * x, int64_t x_col_stride,
+                                    float * dst, int64_t m, int64_t k, int64_t n, void * workspace, size_t workspace_bytes, void * stream);
 /* same through HOST activations/results: H2D(x) -> mul_mat -> D2H(dst), synchronous (end-to-end entry point) */
 B200Q_API int b200q_mul_mat_host(int type, const void * W_planes_dev, const float * x_host, float * dst_host,
                        int64_t m, int64_t k, int64_t n, void * stream);
